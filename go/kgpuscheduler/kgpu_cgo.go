@@ -111,8 +111,9 @@ func (k *handle) scorePair(node int64, gpus int32) (uint32, error) {
 
 // placeBatch: stateful sequential placement (pods in order, the device-side free masks are
 // updated).  dryRun: conflict-free proposals on a scratch copy of the masks, nothing is taken.
-// Same buffers as scoreBatch.
-func (k *handle) placeBatch(pods []int32, dryRun bool) ([]uint64, error) {
+// gang: nil, or one id per pod (0 = on its own; a run of consecutive pods with the same nonzero
+// id is placed all or nothing, kgpu_place_batch_gang).  Same buffers as scoreBatch.
+func (k *handle) placeBatch(pods []int32, gang []int32, dryRun bool) ([]uint64, error) {
 	keys := make([]uint64, len(pods)/4)
 	if len(keys) == 0 {
 		return keys, nil
@@ -121,9 +122,13 @@ func (k *handle) placeBatch(pods []int32, dryRun bool) ([]uint64, error) {
 	if dryRun {
 		flags = C.KGPU_PLACE_DRY_RUN
 	}
-	if rc := C.kgpu_place_batch_ex(k.h, (*C.int32_t)(unsafe.Pointer(&pods[0])), C.int64_t(len(keys)),
+	var g *C.int32_t
+	if gang != nil {
+		g = (*C.int32_t)(unsafe.Pointer(&gang[0]))
+	}
+	if rc := C.kgpu_place_batch_gang(k.h, (*C.int32_t)(unsafe.Pointer(&pods[0])), g, C.int64_t(len(keys)),
 		(*C.uint64_t)(unsafe.Pointer(&keys[0])), flags); rc != C.KGPU_OK {
-		return nil, k.err("kgpu_place_batch_ex")
+		return nil, k.err("kgpu_place_batch_gang")
 	}
 	return keys, nil
 }

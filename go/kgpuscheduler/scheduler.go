@@ -170,25 +170,84 @@ func podGPUs(podInfo *types.PodInfo) int32 { // gpu.go:295-303
 	return int32(n)
 }
 
+// GPUGangID: pod-level request (extension); pods of one PlaceBatch / ProposeBatch with the same nonzero value are
+// placed all or nothing.  ScoreBatch ignores it: snapshot scores change no state.
+const GPUGangID = "gpu/gpu-gang-id"
+
+// gangOrder: the device takes a gang as one run of consecutive pods with an int32 id, so ids are renumbered 1, 2, ...
+// in order of first appearance and each member moves up to its gang's first member.  order[i] = the caller's index of
+// the pod at device position i; gang is nil when no pod carries an id.
+func gangOrder(pods []*types.PodInfo) (order []int, gang []int32) {
+	dense := map[int64]int32{}
+	var members [][]int
+	of := make([]int32, len(pods))
+	for i, p := range pods {
+		id := p.Requests[GPUGangID]
+		if id == 0 {
+			continue
+		}
+		g, ok := dense[id]
+		if !ok {
+			g = int32(len(members) + 1)
+			dense[id] = g
+			members = append(members, nil)
+		}
+		of[i] = g
+		members[g-1] = append(members[g-1], i)
+	}
+	order = make([]int, 0, len(pods))
+	if len(members) == 0 {
+		for i := range pods {
+			order = append(order, i)
+		}
+		return order, nil
+	}
+	gang = make([]int32, 0, len(pods))
+	done := make([]bool, len(members))
+	for i := range pods {
+		switch g := of[i]; {
+		case g == 0:
+			order, gang = append(order, i), append(gang, 0)
+		case !done[g-1]:
+			done[g-1] = true
+			for _, m := range members[g-1] {
+				order, gang = append(order, m), append(gang, g)
+			}
+		}
+	}
+	return order, gang
+}
+
 func (ns *NvidiaGPUScheduler) runBatch(pods []*types.PodInfo, mode int) ([]uint64, error) { // 0 snapshot, 1 sequential, 2 dry run
 	ns.mu.Lock()
 	defer ns.mu.Unlock()
 	if err := ns.flush(); err != nil {
 		return nil, err
 	}
-	req := make([]int32, 4*len(pods))
-	for i, p := range pods {
-		req[4*i], req[4*i+1] = podGPUs(p), int32(i)
+	order, gang := gangOrder(pods)
+	if mode == 0 {
+		for i := range order {
+			order[i] = i
+		}
+		gang = nil
 	}
-	var keys []uint64
+	req := make([]int32, 4*len(pods))
+	for i, p := range order {
+		req[4*i], req[4*i+1] = podGPUs(pods[p]), int32(p)
+	}
+	var dev []uint64
 	var err error
 	if mode == 0 {
-		keys, err = ns.h.scoreBatch(req)
+		dev, err = ns.h.scoreBatch(req)
 	} else {
-		keys, err = ns.h.placeBatch(req, mode == 2)
+		dev, err = ns.h.placeBatch(req, gang, mode == 2)
 	}
 	if err != nil {
 		return nil, err
+	}
+	keys := make([]uint64, len(pods)) // back in the caller's order
+	for i, p := range order {
+		keys[p] = dev[i]
 	}
 	for i, p := range pods {
 		if keys[i] == NoFit {

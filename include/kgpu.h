@@ -20,7 +20,7 @@
  *          batched over every (pod, node) pair instead of one cgo call per pair
  *   kgpu_fit_lookup / kgpu_build_fit_table / kgpu_score_pairs
  *       <- the same PodFitsDevice, called once per (node, pod) by the core: served from a host-side (node, k) table
- *   kgpu_set_free_mask[s] / kgpu_place_batch[_ex] / kgpu_get_free_masks
+ *   kgpu_set_free_mask[s] / kgpu_place_batch[_ex|_gang] / kgpu_get_free_masks
  *       <- TakePodResources / ReturnPodResources       gpuschedulerplugin/gpu_scheduler.go:57-63 (no-ops there)
  *   kgpu_reduce_shards_device
  *       <- (no reference counterpart; the reference is single-process) the final
@@ -185,6 +185,16 @@ int kgpu_place_batch(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out_ke
  * is untouched; commit the accepted ones with kgpu_set_free_masks (TakePodResources). */
 #define KGPU_PLACE_DRY_RUN 1
 int kgpu_place_batch_ex(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out_keys, int flags);
+/* Same with gangs: pods that only work together (the workers of one distributed training job) are placed all or
+ * nothing.  gang[P] holds one id per pod: 0 = the pod is on its own; a GANG is a maximal run of consecutive pods with
+ * the same nonzero id, so list each gang's members next to each other (an id that appears in two separate runs is
+ * KGPU_ERR_INVALID, checked before anything runs).  Pods are placed in order as by kgpu_place_batch_ex; when a member
+ * does not fit (or asks for k outside 0..8), the members of its gang placed before it give their GPUs back, the
+ * members after it are not tried, and every member of the gang gets KGPU_NO_FIT: the free masks are exactly as they
+ * were before the gang's first member, and the pods after the gang see that state.  The result equals
+ * kgpu_place_batch_ex on the batch with every failed gang deleted.  Members may differ in k and min_mem_mib.
+ * gang == NULL is kgpu_place_batch_ex.  Flags, min_mem_mib limits and single-device handles as there. */
+int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, int64_t P, uint64_t *out_keys, int flags);
 /* Copy the current free masks (n = kgpu_num_nodes entries) back to the host. */
 int kgpu_get_free_masks(kgpu_t *h, int32_t *out_free_mask, int64_t n);
 

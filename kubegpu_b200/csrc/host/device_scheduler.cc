@@ -82,6 +82,7 @@ using gpuplugintypes::ResourceGPU;
 
 const char *const GPUTopologyGeneration = "gpu/gpu-generate-topology";
 const char *const GPUMinMemoryMiB = "gpu/gpu-min-memory-mib";
+const char *const GPUGangID = "gpu/gpu-gang-id";
 
 namespace {
 
@@ -568,21 +569,62 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     std::string err = flushNodes();
     if (!err.empty()) return err;
     const size_t P = pods.size();
+    // Gangs (sequential modes only): the device takes a gang as one run of consecutive pods with an int32 id, so the
+    // ids are renumbered 1, 2, ... in order of first appearance (no truncation can merge two gangs) and each member
+    // moves up to its gang's first member.  order[i] = the caller's index of the pod at device position i.
+    std::vector<size_t> order(P);
+    std::vector<int32_t> gang;
+    for (size_t p = 0; p < P; p++) order[p] = p;
+    if (mode != BatchMode::Snapshot) {
+        std::map<int64_t, int32_t> dense;
+        std::vector<std::vector<size_t>> members;
+        std::vector<int32_t> gangOf(P, 0);
+        for (size_t p = 0; p < P; p++) {
+            const int64_t id = getOr0(pods[p]->Requests, GPUGangID);
+            if (id == 0) continue;
+            const auto it = dense.emplace(id, (int32_t)dense.size() + 1).first;
+            if ((size_t)it->second > members.size()) members.emplace_back();
+            gangOf[p] = it->second;
+            members[(size_t)it->second - 1].push_back(p);
+        }
+        if (!members.empty()) {
+            order.clear();
+            gang.reserve(P);
+            std::vector<bool> done(members.size(), false);
+            for (size_t p = 0; p < P; p++) {
+                const int32_t g = gangOf[p];
+                if (g == 0) {
+                    order.push_back(p);
+                    gang.push_back(0);
+                } else if (!done[(size_t)g - 1]) {
+                    done[(size_t)g - 1] = true;
+                    for (size_t m : members[(size_t)g - 1]) {
+                        order.push_back(m);
+                        gang.push_back(g);
+                    }
+                }
+            }
+        }
+    }
     std::vector<int32_t> req(P * 4, 0);
-    for (size_t p = 0; p < P; p++) {
+    for (size_t i = 0; i < P; i++) {
+        const size_t p = order[i];
         types::PodInfo copy = *pods[p];                    // SetGPUReqs mutates; keep the caller's pod intact
         for (auto &c : copy.InitContainers) SetGPUReqs(c.second);
         for (auto &c : copy.RunningContainers) SetGPUReqs(c.second);
         const int64_t k = PodGPUCount(copy);
-        req[p * 4 + 0] = k > 8 ? 9 : (int32_t)k;           // > 8 GPUs never fits one node
-        req[p * 4 + 1] = (int32_t)p;
-        req[p * 4 + 3] = minMemOf(*pods[p]);
+        req[i * 4 + 0] = k > 8 ? 9 : (int32_t)k;           // > 8 GPUs never fits one node
+        req[i * 4 + 1] = (int32_t)p;
+        req[i * 4 + 3] = minMemOf(*pods[p]);
     }
-    std::vector<uint64_t> keys(P, KGPU_NO_FIT);
-    const int rc = mode == BatchMode::Snapshot ? kgpu_score_batch(handle_, req.data(), (int64_t)P, keys.data())
-                                               : kgpu_place_batch_ex(handle_, req.data(), (int64_t)P, keys.data(),
-                                                                     mode == BatchMode::DryRun ? KGPU_PLACE_DRY_RUN : 0);
+    std::vector<uint64_t> dev(P, KGPU_NO_FIT);
+    const int rc = mode == BatchMode::Snapshot ? kgpu_score_batch(handle_, req.data(), (int64_t)P, dev.data())
+                                               : kgpu_place_batch_gang(handle_, req.data(), gang.empty() ? nullptr : gang.data(),
+                                                                       (int64_t)P, dev.data(),
+                                                                       mode == BatchMode::DryRun ? KGPU_PLACE_DRY_RUN : 0);
     if (rc != KGPU_OK) return lastError_ = kgpu_last_error(handle_);
+    std::vector<uint64_t> keys(P, KGPU_NO_FIT);           // back in the caller's order
+    for (size_t i = 0; i < P; i++) keys[order[i]] = dev[i];
     out->assign(P, Placement());
     for (size_t p = 0; p < P; p++) {
         Placement &pl = (*out)[p];

@@ -88,6 +88,10 @@ extern const char *const GPUTopologyGeneration;   // "gpu/gpu-generate-topology"
 // Extension (no reference counterpart): pod-level request "every GPU I get must have at least this
 // many MiB" -- checked against the per-GPU `<gpu>/memory` the node agent advertises.
 extern const char *const GPUMinMemoryMiB;         // "gpu/gpu-min-memory-mib"
+// Extension: pod-level request "I am one of a gang of pods that only work together" (e.g. the workers of one
+// distributed training job).  Pods of one PlaceBatch / ProposeBatch call with the same nonzero value are placed all
+// or nothing; 0 or absent = the pod is on its own.
+extern const char *const GPUGangID;               // "gpu/gpu-gang-id"
 
 // ---- gpu.go, function for function ------------------------------------------------
 types::ResourceList TranslateGPUResources(int64_t neededGPUs, const types::ResourceList &nodeResources,
@@ -170,15 +174,20 @@ public:
     // the two group levels).  Fills *nodeInfo like the agent's UpdateNodeInfo.  "" or error text.
     std::string AddNodeFromGpusInfo(const std::string &nodeName, const std::string &gpusInfoJSON, bool useNVML,
                                     types::NodeInfo *nodeInfo);
-    // Score a whole scheduling cycle in one kernel launch: best node + GPU set per pod.
+    // Score a whole scheduling cycle in one kernel launch: best node + GPU set per pod.  Gang ids are ignored:
+    // snapshot scores change no state, so there is nothing to keep all or nothing.
     std::string ScoreBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out);
     // Place a whole cycle IN ORDER on the device: each pod takes its GPUs before the next one is
     // scored (K3).  The placements are remembered like ScoreBatch's and the usage is recorded, so a
-    // later PodAllocate / ReturnPodResources works on them.
+    // later PodAllocate / ReturnPodResources works on them.  Gangs (GPUGangID): every member is placed right after
+    // the gang's first member in the batch (the others keep their order); if one member does not fit, the whole gang
+    // gets fits = false, takes nothing, and the pods after it are placed as if it had not been in the batch.  `out`
+    // is in the caller's order.
     std::string PlaceBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out);
     // Conflict-free PROPOSALS for a whole cycle: like PlaceBatch (each pod sees the GPUs the pods before it would
     // take) but on a scratch copy of the device state -- nothing is taken until TakePodResources commits a pod.
     // This is the conflict resolution ScoreBatch lacks: its snapshot scores hand every pod of equal k the same GPUs.
+    // Gangs as in PlaceBatch.
     std::string ProposeBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out);
     std::string LastError() const { return lastError_; }
     const TreeCache &cache() const { return cache_; }

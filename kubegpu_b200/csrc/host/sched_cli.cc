@@ -10,12 +10,13 @@
 //   addnode NAME KUBEALLOC [key=val ...]        AddNode with Allocatable = {key: val}
 //   rmnode NAME                                 RemoveNode
 //   topo NAME v0 .. v63                         SetNodeTopology (extension)
-//   pod NAME [topogen=V] [minmem=MiB] {run|init CNAME req=N [kube=N] [dev:key=val ...]}...
+//   pod NAME [topogen=V] [minmem=MiB] [gang=ID] {run|init CNAME req=N [kube=N] [dev:key=val ...]}...
 //   fits NODE POD                               PodFitsDevice  -> fits/score + rewritten requests
 //   allocate NODE POD                           PodAllocate    -> error text + AllocateFrom
 //   take POD | return POD                       TakePodResources / ReturnPodResources
 //   scorebatch POD...                           ScoreBatch (GPU)
 //   placebatch POD...                           PlaceBatch (GPU, sequential, takes the GPUs)
+//   proposebatch POD...                         ProposeBatch (GPU, sequential on a scratch copy, takes nothing)
 //   addjson NAME FILE [nvml]                    AddNodeFromGpusInfo (node agent JSON), dumps names + matrix
 //   visible POD                                 NVIDIA_VISIBLE_DEVICES per container (node agent Allocate)
 //   cache                                       dump the tree cache
@@ -141,6 +142,8 @@ int main(int argc, char **argv) {
                     pod.Requests[GPUTopologyGeneration] = atoll(tok.c_str() + 8);
                 } else if (tok.compare(0, 7, "minmem=") == 0) {
                     pod.Requests[GPUMinMemoryMiB] = atoll(tok.c_str() + 7);
+                } else if (tok.compare(0, 5, "gang=") == 0) {
+                    pod.Requests[GPUGangID] = atoll(tok.c_str() + 5);
                 } else if (cur && tok.compare(0, 4, "req=") == 0) {
                     cur->Requests[gpuplugintypes::ResourceGPU] = atoll(tok.c_str() + 4);
                 } else if (cur && tok.compare(0, 5, "kube=") == 0) {

@@ -12,6 +12,7 @@
 #include <cstring>
 #include <mutex>
 #include <string>
+#include <unordered_set>
 #include <vector>
 
 #include "multi_device.h"
@@ -72,6 +73,7 @@ struct kgpu_shard {
     int64_t n = 0, cap = 0;
     int64_t node_id_base = 0;
     int32_t *d_pods = nullptr;       // [pcap][4]
+    int32_t *d_gang = nullptr;       // [pcap] kgpu_place_batch_gang: gang id per pod
     unsigned long long *d_keys = nullptr;    // [pcap]
     unsigned long long *d_gather = nullptr;  // [ndev][pcap] (multi-device only)
     unsigned long long *d_bestk = nullptr;   // [9] memo variant
@@ -158,10 +160,12 @@ int ensure_pod_capacity(kgpu_ctx *h, kgpu_shard &s, int64_t P) {
     int64_t cap = std::max<int64_t>(1024, P + P / 4);
     KGPU_CUDA(h, cudaSetDevice(s.dev));
     if (s.d_pods) cudaFree(s.d_pods);
+    if (s.d_gang) cudaFree(s.d_gang);
     if (s.d_keys) cudaFree(s.d_keys);
     if (s.d_gather) cudaFree(s.d_gather);
-    s.d_pods = nullptr; s.d_keys = nullptr; s.d_gather = nullptr; s.pcap = 0;
+    s.d_pods = nullptr; s.d_gang = nullptr; s.d_keys = nullptr; s.d_gather = nullptr; s.pcap = 0;
     KGPU_CUDA(h, cudaMalloc(&s.d_pods, (size_t)cap * 16));
+    KGPU_CUDA(h, cudaMalloc(&s.d_gang, (size_t)cap * 4));
     KGPU_CUDA(h, cudaMalloc(&s.d_keys, (size_t)cap * 8));
     if (h->shards.size() > 1) KGPU_CUDA(h, cudaMalloc(&s.d_gather, (size_t)cap * 8 * h->shards.size()));
     s.pcap = cap;
@@ -523,6 +527,7 @@ void free_shard(kgpu_shard &s) {
     if (s.d_query) cudaFree(s.d_query);
     if (s.d_qout) cudaFree(s.d_qout);
     if (s.d_pods) cudaFree(s.d_pods);
+    if (s.d_gang) cudaFree(s.d_gang);
     if (s.d_keys) cudaFree(s.d_keys);
     if (s.d_gather) cudaFree(s.d_gather);
     if (s.d_bestk) cudaFree(s.d_bestk);
@@ -882,11 +887,24 @@ int kgpu_place_batch(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out_ke
 }
 
 int kgpu_place_batch_ex(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out_keys, int flags) {
+    return kgpu_place_batch_gang(h, pods, nullptr, P, out_keys, flags);
+}
+
+int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, int64_t P, uint64_t *out_keys, int flags) {
     if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_place_batch: NULL handle");
     std::lock_guard<std::mutex> g(h->mu);
     if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_place_batch: needs a single-device handle");
     if (P < 0 || (P > 0 && (!pods || !out_keys))) return fail(h, KGPU_ERR_INVALID, "kgpu_place_batch: bad arguments");
     if (P == 0) return KGPU_OK;
+    if (gang) {                            // a gang is ONE run of consecutive pods: the kernel only looks at neighbours
+        std::unordered_set<int32_t> seen;
+        for (int64_t p = 0; p < P; p++) {
+            if (gang[p] == 0 || (p > 0 && gang[p - 1] == gang[p])) continue;
+            if (!seen.insert(gang[p]).second)
+                return fail(h, KGPU_ERR_INVALID, "kgpu_place_batch_gang: gang id %d appears in two separate runs (again at pod %lld)",
+                            gang[p], (long long)p);
+        }
+    }
     // the batch's distinct memory requirements are the views the sequential kernels keep tables for
     kgpu::PlaceViews views;
     memset(&views, 0, sizeof views);
@@ -906,6 +924,7 @@ int kgpu_place_batch_ex(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out
     if (rc != KGPU_OK) return rc;
     KGPU_CUDA(h, cudaSetDevice(s.dev));
     KGPU_CUDA(h, cudaMemcpyAsync(s.d_pods, pods, (size_t)P * 16, cudaMemcpyHostToDevice, s.stream));
+    if (gang) KGPU_CUDA(h, cudaMemcpyAsync(s.d_gang, gang, (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
     const bool dry = (flags & KGPU_PLACE_DRY_RUN) != 0;
     int32_t *d_free = s.d_free;
     if (dry && s.n > 0) {                  // place on a scratch copy of the masks: conflict-free proposals, nothing taken
@@ -942,12 +961,21 @@ int kgpu_place_batch_ex(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out
         kgpu::place_half_tables<<<(unsigned)std::min<int64_t>((s.n + 3) / 4, (int64_t)s.sm_count * 16), 128, 0, s.stream>>>(
             s.d_topo, s.n, W, s.d_half);
         h->launches++;
-        static const cudaError_t place_attr = cudaFuncSetAttribute(kgpu::place_sequential, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                                   (int)kgpu::PLACE_DYN_SMEM);
-        KGPU_CUDA(h, place_attr);
-        kgpu::place_sequential<<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base,
-                                                                        reinterpret_cast<const int4 *>(s.d_pods), P, W, views,
-                                                                        s.d_nodebest, s.d_tilebest, T, s.d_half, s.d_keys);
+        if (gang) {
+            static const cudaError_t place_gang_attr = cudaFuncSetAttribute(
+                kgpu::place_sequential<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kgpu::PLACE_DYN_SMEM);
+            KGPU_CUDA(h, place_gang_attr);
+            kgpu::place_sequential<true><<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(
+                s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base, reinterpret_cast<const int4 *>(s.d_pods), P, W, views,
+                s.d_nodebest, s.d_tilebest, T, s.d_half, s.d_keys, s.d_gang);
+        } else {
+            static const cudaError_t place_attr = cudaFuncSetAttribute(kgpu::place_sequential<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                                       (int)kgpu::PLACE_DYN_SMEM);
+            KGPU_CUDA(h, place_attr);
+            kgpu::place_sequential<false><<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base,
+                                                                                   reinterpret_cast<const int4 *>(s.d_pods), P, W, views,
+                                                                                   s.d_nodebest, s.d_tilebest, T, s.d_half, s.d_keys);
+        }
         h->launches += 2;
         if (!dry) {
             s.order_dirty = true;        // the free masks have changed on the device: re-sort + recompact lazily

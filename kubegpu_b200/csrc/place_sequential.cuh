@@ -216,11 +216,21 @@ constexpr size_t PLACE_DYN_SMEM = 2 * (size_t)PLACE_SUPER_CAP * sizeof(unsigned 
 //      REDUX over a 32-bit composite (cost << 15 | node offset << 8 | S; cost < 2^17); supertile minimum: two.
 //   3. ONE barrier.
 // Pod requests are staged PLACE_POD_CHUNK at a time; indices are 32-bit shifts (supertiles are 32 << j tiles).
+//
+// Gangs (GANG = true, gang[P] != nullptr): a maximal run of consecutive pods with the same nonzero gang id is placed
+// all or nothing.  When a member misses (NO_FIT or k outside 0..8), the members placed before it give their GPUs back,
+// last first: each undo is step 2 with free mask c_fm | S instead of c_fm & ~S, i.e. one more epoch, so the double-
+// buffered supertile minima and the per-warp caches need no special case.  The members' keys are read back from
+// keys[] (tid 0 wrote them; the barrier before the walk makes them visible), so a gang may cross a staging chunk.
+// Members after the miss are not tried; every member's key becomes NO_FIT.  The host guarantees that no id appears
+// in two separate runs.  GANG = false is the plain kernel, with no gang bookkeeping on its chain.
+template <bool GANG = false>
 __global__ void __launch_bounds__(PLACE_THREADS, 1)
 place_sequential(const int32_t *__restrict__ topo, int32_t *__restrict__ free_mask, const int32_t *__restrict__ gpu_mem,
                  int64_t N, int64_t Npad, int64_t node_id_base, const int4 *__restrict__ pods4, int64_t P, Weights W,
                  PlaceViews views, uint32_t *__restrict__ nodebest, unsigned long long *__restrict__ tilebest, int64_t T,
-                 const int32_t *__restrict__ half_all /*[N][96], place_half_tables*/, unsigned long long *__restrict__ keys) {
+                 const int32_t *__restrict__ half_all /*[N][96], place_half_tables*/, unsigned long long *__restrict__ keys,
+                 const int32_t *__restrict__ gang = nullptr /*[P], GANG only*/) {
     __shared__ int32_t sViewMin[PLACE_MAX_VIEWS];                 // static indexing of the kernel parameter only
     __shared__ int32_t sHalf[PLACE_WARPS][PLACE_HALF];            // per warp: the cached node's half tables (node_key_warp)
     __shared__ uint8_t sSub[9][72];                               // the k-subsets of 8 GPUs, increasing
@@ -234,6 +244,7 @@ place_sequential(const int32_t *__restrict__ topo, int32_t *__restrict__ free_ma
     __shared__ int32_t sPendIdx[PLACE_MAX_VIEWS * 9];             // per task: entry still to be written to the other copy
     __shared__ unsigned long long sPendVal[PLACE_MAX_VIEWS * 9];
     __shared__ int4 sPods[PLACE_POD_CHUNK];
+    __shared__ int32_t sGang[GANG ? PLACE_POD_CHUNK : 1];         // gang id of each staged pod (4 KB, GANG only)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int V = views.n;
     const int super_tiles = (int)place_super_tiles(T, V);         // 32 << j
@@ -271,189 +282,232 @@ place_sequential(const int32_t *__restrict__ topo, int32_t *__restrict__ free_ma
 #pragma unroll
     for (int j = 0; j < PLACE_TILE / 32; j++) nbr[j] = INF32;
 
+    int64_t g_first = 0;                                          // GANG, block-uniform: first pod of the current gang,
+    int32_t g_id = 0;                                             // its id (0: the pod is on its own)
+    bool g_failed = false;                                        // and whether one of its members has missed
+
     for (int64_t p0 = 0; p0 < P; p0 += PLACE_POD_CHUNK) {
         const int pn = (int)min((int64_t)PLACE_POD_CHUNK, P - p0);
         __syncthreads();
-        for (int i = tid; i < pn; i += PLACE_THREADS) sPods[i] = __ldg(pods4 + p0 + i);
+        for (int i = tid; i < pn; i += PLACE_THREADS) {
+            sPods[i] = __ldg(pods4 + p0 + i);
+            if constexpr (GANG) sGang[i] = __ldg(gang + p0 + i);
+        }
         __syncthreads();
 #pragma unroll 1
         for (int pi = 0; pi < pn; pi++) {
             const int4 req = sPods[pi];                       // block-uniform
             const int k = req.x;
+            if constexpr (GANG) {
+                const int32_t id = sGang[pi];
+                if (id == 0 || id != g_id) {                  // a pod on its own, or the first member of a gang
+                    g_first = p0 + pi;
+                    g_id = id;
+                    g_failed = false;
+                } else if (g_failed) {                        // a later member of a gang that has failed: not tried
+                    if (tid == 0) keys[p0 + pi] = ~0ull;
+                    continue;
+                }
+            }
+            unsigned long long win = ~0ull;
             if (k < 0 || k > 8) {
                 if (tid == 0) keys[p0 + pi] = ~0ull;
-                continue;
+                if (!GANG || g_id == 0) continue;
+            } else {
+                int v = 0;                                    // the pod's view: the one with its min_mem
+                for (int j = 1; j < V; j++)
+                    if (req.w == sViewMin[j]) v = j;
+                // 1. the winner, by every warp for itself
+                const unsigned long long *sp = sSuper[epoch & 1] + (v * 9 + k) * ST;
+                unsigned long long best = ~0ull;
+                for (int s = lane; s < ST; s += 32) best = min(best, sp[s]);
+                win = warp_min_u64_redux(best);
+                if (tid == 0) keys[p0 + pi] = win;
+                if (win == ~0ull || k == 0)                   // nothing fits / nothing to take (block-uniform)
+                    if (!GANG || win != ~0ull || g_id == 0) continue;
             }
-            int v = 0;                                        // the pod's view: the one with its min_mem
-            for (int j = 1; j < V; j++)
-                if (req.w == sViewMin[j]) v = j;
-            // 1. the winner, by every warp for itself
-            const unsigned long long *sp = sSuper[epoch & 1] + (v * 9 + k) * ST;
-            unsigned long long best = ~0ull;
-            for (int s = lane; s < ST; s += 32) best = min(best, sp[s]);
-            const unsigned long long win = warp_min_u64_redux(best);
-            if (tid == 0) keys[p0 + pi] = win;
-            if (win == ~0ull || k == 0) continue;             // nothing fits / nothing to take (block-uniform)
-
-            // 2. commit and refresh, warp by warp
-            const uint32_t nid = (uint32_t)(win >> 8);
-            const int node = (int)((int64_t)nid - node_id_base);
-            const uint32_t S = (uint32_t)(win & 0xFFull);
-            const int tile = node >> 7, st = tile >> st_shift;
-            static_assert(PLACE_TILE == 128, "tile index is node >> 7");
-            if (warp < min(PLACE_WARPS, ntask)) {
-                const int64_t vk0 = warp;                     // this warp's first (cached) task
-                const bool new_node = node != c_node, new_tile = tile != c_tile;
-                const bool cache_super = super_tiles == 32;
-                const bool new_st = !cache_super || st != c_st;
-                // every global load this pod needs from this warp, issued before anything waits
-                int32_t h0 = 0, h1 = 0, h2 = 0;
-                uint32_t fm_mem = 0;
-                if (new_node) {                               // the winner's half tables: three coalesced loads (L1 if prefetched)
-                    const int32_t *src = half_all + (int64_t)node * PLACE_HALF;
-                    h0 = __ldg(src + lane);
-                    h1 = __ldg(src + lane + 32);
-                    h2 = __ldg(src + lane + 64);
-                    fm_mem = (uint32_t)free_mask[node] & 0xFFu;       // before or after warp 0's write-back: & ~S below either way
-                    c_mem = (gpu_mem != nullptr && lane < 8) ? __ldg(gpu_mem + (int64_t)node * 8 + lane) : 0x7FFFFFFF;
+            // The placement step 2 commits: this pod's (take), or -- GANG, a member has missed -- those of the members
+            // placed before it, last first, each given back (one epoch each).
+            bool take = true;
+            int64_t back = p0 + pi;                           // GANG: the member being given back
+            if constexpr (GANG) {
+                if (win == ~0ull) {
+                    __syncthreads();                          // the members' keys (tid 0 wrote them) are visible
+                    take = false;
+                    while (--back >= g_first && ((win = keys[back]) & 0xFFull) == 0) {}     // k == 0 took nothing
                 }
-                if (new_tile) {
-#pragma unroll
-                    for (int j = 0; j < PLACE_TILE / 32; j++) nbr[j] = nodebest[vk0 * Npad + tile * PLACE_TILE + lane + 32 * j];
-                }
-                unsigned long long sb0 = ~0ull;               // !cache_super: minimum over the supertile's OTHER tiles
-                if (cache_super) {
-                    if (new_st) {
-                        const int t = (st << 5) + lane;
-                        tsr = t < Ti ? tilebest[vk0 * T + t] : ~0ull;
+            }
+#pragma unroll 1
+            while (take || back >= g_first) {
+                // 2. commit and refresh, warp by warp: the winner node loses S (take) or, undoing a gang member, gets S back
+                const uint32_t nid = (uint32_t)(win >> 8);
+                const int node = (int)((int64_t)nid - node_id_base);
+                const uint32_t S = (uint32_t)(win & 0xFFull);
+                const int tile = node >> 7, st = tile >> st_shift;
+                static_assert(PLACE_TILE == 128, "tile index is node >> 7");
+                if (warp < min(PLACE_WARPS, ntask)) {
+                    const int64_t vk0 = warp;                     // this warp's first (cached) task
+                    const bool new_node = node != c_node, new_tile = tile != c_tile;
+                    const bool cache_super = super_tiles == 32;
+                    const bool new_st = !cache_super || st != c_st;
+                    // every global load this pod needs from this warp, issued before anything waits
+                    int32_t h0 = 0, h1 = 0, h2 = 0;
+                    uint32_t fm_mem = 0;
+                    if (new_node) {                               // the winner's half tables: three coalesced loads (L1 if prefetched)
+                        const int32_t *src = half_all + (int64_t)node * PLACE_HALF;
+                        h0 = __ldg(src + lane);
+                        h1 = __ldg(src + lane + 32);
+                        h2 = __ldg(src + lane + 64);
+                        fm_mem = (uint32_t)free_mask[node] & 0xFFu;       // before or after warp 0's write-back: & ~S (| S) below either way
+                        c_mem = (gpu_mem != nullptr && lane < 8) ? __ldg(gpu_mem + (int64_t)node * 8 + lane) : 0x7FFFFFFF;
                     }
-                } else {
-                    for (int t = (st << st_shift) + lane; t < min(Ti, (st + 1) << st_shift); t += 32)
-                        if (t != tile) sb0 = min(sb0, tilebest[vk0 * T + t]);
-                }
-                int32_t *half = sHalf[warp];
-                if (new_node) {
-                    __syncwarp();
-                    half[lane] = h0;
-                    half[lane + 32] = h1;
-                    half[lane + 64] = h2;
-                    __syncwarp();
-                    c_fm = fm_mem;
-                    c_node = node;
-                }
-                c_tile = tile;
-                c_st = st;
-                const uint32_t fm = c_fm & ~S;
-                c_fm = fm;
-                if (warp == 0 && lane == 0) free_mask[node] = (int32_t)fm;
-                for (int task = warp; task < ntask; task += PLACE_WARPS) {
-                    const int tv = task / 9, tk = task - tv * 9;
-                    const int64_t vk = task;
-                    const bool cached = task == warp;
-                    uint32_t nb[PLACE_TILE / 32];
-                    unsigned long long sb = sb0;
-                    if (!cached) {                            // more tasks than warps (several views): load now
+                    if (new_tile) {
 #pragma unroll
-                        for (int j = 0; j < PLACE_TILE / 32; j++) nb[j] = nodebest[vk * Npad + tile * PLACE_TILE + lane + 32 * j];
-                        sb = ~0ull;
-                        for (int t = (st << st_shift) + lane; t < min(Ti, (st + 1) << st_shift); t += 32)
-                            if (t != tile) sb = min(sb, tilebest[vk * T + t]);
+                        for (int j = 0; j < PLACE_TILE / 32; j++) nbr[j] = nodebest[vk0 * Npad + tile * PLACE_TILE + lane + 32 * j];
                     }
-                    const uint32_t ok = tv == 0 ? 0xFFu : (__ballot_sync(0xFFFFFFFFu, c_mem >= sViewMin[tv]) & 0xFFu);
-                    const uint32_t nk = node_key_warp(tk, half, fm & ok, lane, sSub[tk], sNsub[tk]);
-                    // tile minimum: 32-bit composite cost << 15 | node offset << 8 | S (cost <= 28 * 4095 < 2^17)
-                    uint32_t m = INF32;
-#pragma unroll
-                    for (int j = 0; j < PLACE_TILE / 32; j++) {
-                        const int off = lane + 32 * j;
-                        uint32_t key = cached ? nbr[j] : nb[j];
-                        if (tile * PLACE_TILE + off == node) {
-                            key = nk;
-                            if (cached) nbr[j] = nk;
+                    unsigned long long sb0 = ~0ull;               // !cache_super: minimum over the supertile's OTHER tiles
+                    if (cache_super) {
+                        if (new_st) {
+                            const int t = (st << 5) + lane;
+                            tsr = t < Ti ? tilebest[vk0 * T + t] : ~0ull;
                         }
-                        if (key != INF32) m = min(m, ((key >> 8) << 15) | ((uint32_t)off << 8) | (key & 0xFFu));
-                    }
-                    m = __reduce_min_sync(0xFFFFFFFFu, m);
-                    const unsigned long long tb =
-                        m == INF32 ? ~0ull
-                                   : (((unsigned long long)(m >> 15) << 40) |
-                                      ((unsigned long long)(node_id_base + (int64_t)tile * PLACE_TILE + ((m >> 8) & 127u)) << 8) | (m & 0xFFu));
-                    if (cached && cache_super) {
-                        if (lane == (tile & 31)) tsr = tb;
-                        sb = warp_min_u64_redux(tsr);
                     } else {
-                        sb = warp_min_u64_redux(min(sb, tb));
+                        for (int t = (st << st_shift) + lane; t < min(Ti, (st + 1) << st_shift); t += 32)
+                            if (t != tile) sb0 = min(sb0, tilebest[vk0 * T + t]);
                     }
-                    if (lane == 0) {
-                        nodebest[vk * Npad + node] = nk;
-                        tilebest[vk * T + tile] = tb;
-                        // last epoch's refreshed minimum reaches the copy the winners are read from NEXT epoch ...
-                        const int pe = sPendIdx[task];
-                        if (pe >= 0) sSuper[(epoch + 1) & 1][pe] = sPendVal[task];
-                        // ... and this epoch's goes to that copy now, to the other one an epoch later
-                        sSuper[(epoch + 1) & 1][vk * ST + st] = sb;
-                        sPendIdx[task] = (int)(vk * ST + st);
-                        sPendVal[task] = sb;
+                    int32_t *half = sHalf[warp];
+                    if (new_node) {
+                        __syncwarp();
+                        half[lane] = h0;
+                        half[lane + 32] = h1;
+                        half[lane + 64] = h2;
+                        __syncwarp();
+                        c_fm = fm_mem;
+                        c_node = node;
                     }
+                    c_tile = tile;
+                    c_st = st;
+                    const uint32_t fm = take ? (c_fm & ~S) : (c_fm | S);
+                    c_fm = fm;
+                    if (warp == 0 && lane == 0) free_mask[node] = (int32_t)fm;
+                    for (int task = warp; task < ntask; task += PLACE_WARPS) {
+                        const int tv = task / 9, tk = task - tv * 9;
+                        const int64_t vk = task;
+                        const bool cached = task == warp;
+                        uint32_t nb[PLACE_TILE / 32];
+                        unsigned long long sb = sb0;
+                        if (!cached) {                            // more tasks than warps (several views): load now
+#pragma unroll
+                            for (int j = 0; j < PLACE_TILE / 32; j++) nb[j] = nodebest[vk * Npad + tile * PLACE_TILE + lane + 32 * j];
+                            sb = ~0ull;
+                            for (int t = (st << st_shift) + lane; t < min(Ti, (st + 1) << st_shift); t += 32)
+                                if (t != tile) sb = min(sb, tilebest[vk * T + t]);
+                        }
+                        const uint32_t ok = tv == 0 ? 0xFFu : (__ballot_sync(0xFFFFFFFFu, c_mem >= sViewMin[tv]) & 0xFFu);
+                        const uint32_t nk = node_key_warp(tk, half, fm & ok, lane, sSub[tk], sNsub[tk]);
+                        // tile minimum: 32-bit composite cost << 15 | node offset << 8 | S (cost <= 28 * 4095 < 2^17)
+                        uint32_t m = INF32;
+#pragma unroll
+                        for (int j = 0; j < PLACE_TILE / 32; j++) {
+                            const int off = lane + 32 * j;
+                            uint32_t key = cached ? nbr[j] : nb[j];
+                            if (tile * PLACE_TILE + off == node) {
+                                key = nk;
+                                if (cached) nbr[j] = nk;
+                            }
+                            if (key != INF32) m = min(m, ((key >> 8) << 15) | ((uint32_t)off << 8) | (key & 0xFFu));
+                        }
+                        m = __reduce_min_sync(0xFFFFFFFFu, m);
+                        const unsigned long long tb =
+                            m == INF32 ? ~0ull
+                                       : (((unsigned long long)(m >> 15) << 40) |
+                                          ((unsigned long long)(node_id_base + (int64_t)tile * PLACE_TILE + ((m >> 8) & 127u)) << 8) | (m & 0xFFu));
+                        if (cached && cache_super) {
+                            if (lane == (tile & 31)) tsr = tb;
+                            sb = warp_min_u64_redux(tsr);
+                        } else {
+                            sb = warp_min_u64_redux(min(sb, tb));
+                        }
+                        if (lane == 0) {
+                            nodebest[vk * Npad + node] = nk;
+                            tilebest[vk * T + tile] = tb;
+                            // last epoch's refreshed minimum reaches the copy the winners are read from NEXT epoch ...
+                            const int pe = sPendIdx[task];
+                            if (pe >= 0) sSuper[(epoch + 1) & 1][pe] = sPendVal[task];
+                            // ... and this epoch's goes to that copy now, to the other one an epoch later
+                            sSuper[(epoch + 1) & 1][vk * ST + st] = sb;
+                            sPendIdx[task] = (int)(vk * ST + st);
+                            sPendVal[task] = sb;
+                        }
 #ifndef KGPU_PLACE_PREFETCH
 #define KGPU_PLACE_PREFETCH 0      // 0: off (default), 1: half tables + mask, 2: + the node-key row of the candidate's tile.  Off because on C2 the candidate search and the prefetch instructions on the chain cost more than the L1 hits save (not re-measured on the H100)
 #endif
-                    if (cached && KGPU_PLACE_PREFETCH) {
-                        // The next winner for THIS warp's (view, k), unless another pod changes that first: the minimum of
-                        // the row this warp has just brought up to date (copy (epoch + 1) & 1 is written by this warp
-                        // only).  Every second pod opens a node nobody has touched yet (a node holds at most 8 GPUs'
-                        // worth of pods), so its half tables and mask are brought into this SM's L1 now, off the chain.
-                        __syncwarp();
-                        const unsigned long long *row = sSuper[(epoch + 1) & 1] + vk * ST;
-                        unsigned long long cb = ~0ull;
-                        for (int s2 = lane; s2 < ST; s2 += 32) cb = min(cb, row[s2]);
-                        cb = warp_min_u64_redux(cb);
-                        if (cb != ~0ull) {
-                            const int64_t cand = (int64_t)((cb >> 8) & 0xFFFFFFFFull) - node_id_base;
-                            if (cand != c_node) {
-                                if (lane < 4) prefetch_l1(lane < 3 ? (const void *)(half_all + cand * PLACE_HALF + 32 * lane) : (const void *)(free_mask + cand));
-                                if (KGPU_PLACE_PREFETCH >= 2 && lane >= 4 && lane < 8)
-                                    prefetch_l1(nodebest + vk * Npad + (cand & ~(int64_t)127) + 32 * (lane - 4));
+                        if (cached && KGPU_PLACE_PREFETCH) {
+                            // The next winner for THIS warp's (view, k), unless another pod changes that first: the minimum of
+                            // the row this warp has just brought up to date (copy (epoch + 1) & 1 is written by this warp
+                            // only).  Every second pod opens a node nobody has touched yet (a node holds at most 8 GPUs'
+                            // worth of pods), so its half tables and mask are brought into this SM's L1 now, off the chain.
+                            __syncwarp();
+                            const unsigned long long *row = sSuper[(epoch + 1) & 1] + vk * ST;
+                            unsigned long long cb = ~0ull;
+                            for (int s2 = lane; s2 < ST; s2 += 32) cb = min(cb, row[s2]);
+                            cb = warp_min_u64_redux(cb);
+                            if (cb != ~0ull) {
+                                const int64_t cand = (int64_t)((cb >> 8) & 0xFFFFFFFFull) - node_id_base;
+                                if (cand != c_node) {
+                                    if (lane < 4) prefetch_l1(lane < 3 ? (const void *)(half_all + cand * PLACE_HALF + 32 * lane) : (const void *)(free_mask + cand));
+                                    if (KGPU_PLACE_PREFETCH >= 2 && lane >= 4 && lane < 8)
+                                        prefetch_l1(nodebest + vk * Npad + (cand & ~(int64_t)127) + 32 * (lane - 4));
+                                }
                             }
                         }
                     }
                 }
-            }
 #ifndef KGPU_PLACE_HELPER
 #define KGPU_PLACE_HELPER 1        // a warp without a task (warp 9 with one view) prefetches the NEXT pod's candidate into L1
 #endif
-            else if (KGPU_PLACE_HELPER && pi + 1 < pn) {
-                // Off the chain: the next pod's winner under the state BEFORE this pod's update is its winner afterwards
-                // too unless it is this pod's node (a placement only RAISES the keys of one node).  While the other warps
-                // refresh, bring what they will load for that node into this SM's L1: its half tables and mask, and for
-                // every task the node-key row of its tile and the tile minima of its supertile.
-                const int4 rq = sPods[pi + 1];
-                const int k2 = rq.x;
-                if (k2 >= 1 && k2 <= 8) {
-                    int v2 = 0;
-                    for (int j = 1; j < V; j++)
-                        if (rq.w == sViewMin[j]) v2 = j;
-                    const unsigned long long *sp2 = sSuper[epoch & 1] + (v2 * 9 + k2) * ST;
-                    unsigned long long b2 = ~0ull;
-                    for (int s2 = lane; s2 < ST; s2 += 32) b2 = min(b2, sp2[s2]);
-                    b2 = warp_min_u64_redux(b2);
-                    const int64_t cand = (int64_t)((b2 >> 8) & 0xFFFFFFFFull) - node_id_base;
-                    if (b2 != ~0ull && cand != node) {
-                        const int64_t ctile = cand >> 7, cst = ctile >> st_shift;
-                        const int rows = ntask * 4, mins = ntask * 2;       // 128-byte lines: 4 per node-key row, 2 per 32 tile minima
-                        for (int e = lane; e < 4 + rows + mins; e += 32) {
-                            const void *q;
-                            if (e < 3) q = half_all + cand * PLACE_HALF + 32 * e;
-                            else if (e == 3) q = free_mask + cand;
-                            else if (e < 4 + rows) { const int t = (e - 4) >> 2, j = (e - 4) & 3; q = nodebest + (int64_t)t * Npad + ctile * PLACE_TILE + 32 * j; }
-                            else { const int t = (e - 4 - rows) >> 1, j = (e - 4 - rows) & 1; q = tilebest + (int64_t)t * T + min((int64_t)Ti - 1, (cst << st_shift) + 16 * j); }
-                            prefetch_l1(q);
+                else if (KGPU_PLACE_HELPER && take && pi + 1 < pn) {
+                    // Off the chain: the next pod's winner under the state BEFORE this pod's update is its winner afterwards
+                    // too unless it is this pod's node (a placement only RAISES the keys of one node).  While the other warps
+                    // refresh, bring what they will load for that node into this SM's L1: its half tables and mask, and for
+                    // every task the node-key row of its tile and the tile minima of its supertile.
+                    const int4 rq = sPods[pi + 1];
+                    const int k2 = rq.x;
+                    if (k2 >= 1 && k2 <= 8) {
+                        int v2 = 0;
+                        for (int j = 1; j < V; j++)
+                            if (rq.w == sViewMin[j]) v2 = j;
+                        const unsigned long long *sp2 = sSuper[epoch & 1] + (v2 * 9 + k2) * ST;
+                        unsigned long long b2 = ~0ull;
+                        for (int s2 = lane; s2 < ST; s2 += 32) b2 = min(b2, sp2[s2]);
+                        b2 = warp_min_u64_redux(b2);
+                        const int64_t cand = (int64_t)((b2 >> 8) & 0xFFFFFFFFull) - node_id_base;
+                        if (b2 != ~0ull && cand != node) {
+                            const int64_t ctile = cand >> 7, cst = ctile >> st_shift;
+                            const int rows = ntask * 4, mins = ntask * 2;       // 128-byte lines: 4 per node-key row, 2 per 32 tile minima
+                            for (int e = lane; e < 4 + rows + mins; e += 32) {
+                                const void *q;
+                                if (e < 3) q = half_all + cand * PLACE_HALF + 32 * e;
+                                else if (e == 3) q = free_mask + cand;
+                                else if (e < 4 + rows) { const int t = (e - 4) >> 2, j = (e - 4) & 3; q = nodebest + (int64_t)t * Npad + ctile * PLACE_TILE + 32 * j; }
+                                else { const int t = (e - 4 - rows) >> 1, j = (e - 4 - rows) & 1; q = tilebest + (int64_t)t * T + min((int64_t)Ti - 1, (cst << st_shift) + 16 * j); }
+                                prefetch_l1(q);
+                            }
                         }
                     }
                 }
+                epoch++;
+                __syncthreads();
+                if (take) break;
+                while (--back >= g_first && ((win = keys[back]) & 0xFFull) == 0) {}
             }
-            epoch++;
-            __syncthreads();
+            if constexpr (GANG) {
+                if (!take) {                                  // every member gets NO_FIT
+                    __syncthreads();                          // once every thread has read the keys
+                    for (int64_t m = g_first + tid; m <= p0 + pi; m += PLACE_THREADS) keys[m] = ~0ull;
+                    g_failed = true;
+                }
+            }
         }
     }
 }

@@ -146,14 +146,24 @@ class Scorer:
         self._check(self._L.kgpu_score_batch(self._h, pods.ctypes.data, P, out.ctypes.data))
         return out
 
-    def place_batch(self, pods, out: Optional[np.ndarray] = None, dry_run: bool = False) -> np.ndarray:
+    def place_batch(self, pods, out: Optional[np.ndarray] = None, dry_run: bool = False, gang=None) -> np.ndarray:
         """Stateful sequential placement: pods in order, each takes its GPUs (device free masks change).
-        dry_run: conflict-free proposals on a scratch copy of the masks, the handle's state is untouched."""
+        dry_run: conflict-free proposals on a scratch copy of the masks, the handle's state is untouched.
+        gang: int32[P] gang ids, 0 = the pod is on its own.  A run of consecutive pods with the same nonzero id
+        is placed all or nothing: if a member does not fit, the members before it give their GPUs back and the
+        whole gang gets NO_FIT.  An id in two separate runs raises KgpuError (ERR_INVALID)."""
         pods = _i32(pods)
         P = pods.size // 4
         if out is None:
             out = np.empty(P, dtype=np.uint64)
-        self._check(self._L.kgpu_place_batch_ex(self._h, pods.ctypes.data, P, out.ctypes.data, _lib.PLACE_DRY_RUN if dry_run else 0))
+        flags = _lib.PLACE_DRY_RUN if dry_run else 0
+        if gang is None:
+            self._check(self._L.kgpu_place_batch_ex(self._h, pods.ctypes.data, P, out.ctypes.data, flags))
+            return out
+        gang = _i32(gang)
+        if gang.size != P:
+            raise ValueError("gang must hold one id per pod")
+        self._check(self._L.kgpu_place_batch_gang(self._h, pods.ctypes.data, gang.ctypes.data, P, out.ctypes.data, flags))
         return out
 
     def get_free_masks(self) -> np.ndarray:

@@ -21,6 +21,7 @@ SEED_C2 = 0xB2000001
 SEED_C3 = 0xB2000002
 SEED_C4 = 0xB2000003
 SEED_C5 = 0xB2000005
+SEED_GANGS = 0xB2000007
 
 _M64 = np.uint64(0xFFFFFFFFFFFFFFFF)
 
@@ -151,3 +152,27 @@ def gen_c6(N: int = 100_000, P: int = 10_000, seed: int = SEED_C6, node_start: i
     mem = gen_gpu_memory(N, seed, node_start)
     pods[:, 3] = np.array(POD_MIN_MEM_CHOICES_MIB, dtype=np.int32)[rand_below(seed, 14, P, len(POD_MIN_MEM_CHOICES_MIB))]
     return topo, free, mem, pods
+
+
+def gen_gangs(N: int = 100_000, P: int = 10_000, seed: int = SEED_GANGS, gang_start: float = 0.1):
+    """C2's cluster and pod stream, with distributed training jobs mixed in: at each pod that is not yet in a gang,
+    a gang starts with probability ``gang_start`` (default: about a third of the pods end up in gangs).  A gang has
+    2..8 members that all want the same k in {4, 8} and sit next to each other; ids are 1, 2, ... in order.  At C2's
+    size the nodes with 8 free GPUs run out early, so many k = 8 gangs fail part way.
+    Returns (topo, free, pods, gang[P])."""
+    topo, free, pods = gen_c2(N, P, seed)
+    start = rand_below(seed, 21, P, 1 << 20) < int(gang_start * (1 << 20))
+    size = 2 + rand_below(seed, 22, P, 7)
+    kg = np.array([4, 8], dtype=np.int32)[rand_below(seed, 23, P, 2)]
+    gang = np.zeros(P, dtype=np.int32)
+    p, gid = 0, 0
+    while p < P:
+        if start[p]:
+            gid += 1
+            end = min(P, p + int(size[p]))
+            gang[p:end] = gid
+            pods[p:end, 0] = kg[p]
+            p = end
+        else:
+            p += 1
+    return topo, free, pods, gang
