@@ -143,3 +143,43 @@ func (k *handle) freeMasks(n int64) ([]int32, error) {
 	}
 	return out, nil
 }
+
+// uploadHolders: the whole holder table, 8 entries per node (-1, or level<<3 | owner), n = the node count.
+func (k *handle) uploadHolders(holders []int32) error {
+	n := len(holders) / 8
+	var p *C.int32_t
+	if n > 0 {
+		p = (*C.int32_t)(unsafe.Pointer(&holders[0]))
+	}
+	if rc := C.kgpu_upload_holders(k.h, p, C.int64_t(n)); rc != C.KGPU_OK {
+		return k.err("kgpu_upload_holders")
+	}
+	return nil
+}
+
+// setHolders: replace the rows of nodes idx (holders holds 8 entries per index) in one copy; the last row wins.
+func (k *handle) setHolders(idx []int64, holders []int32) error {
+	if len(idx) == 0 {
+		return nil
+	}
+	if rc := C.kgpu_set_holders(k.h, (*C.int64_t)(unsafe.Pointer(&idx[0])), (*C.int32_t)(unsafe.Pointer(&holders[0])),
+		C.int64_t(len(idx))); rc != C.KGPU_OK {
+		return k.err("kgpu_set_holders")
+	}
+	return nil
+}
+
+// preemptBatch: for each pod the best placement when running pods of a lower level (lvl, 0..15) may be evicted,
+// and the owner mask of its victims on the key's node (kgpu_preempt_batch).  Same pod buffer as scoreBatch.
+func (k *handle) preemptBatch(pods []int32, lvl []int32) ([]uint64, []uint32, error) {
+	keys := make([]uint64, len(pods)/4)
+	victims := make([]uint32, len(keys))
+	if len(keys) == 0 {
+		return keys, victims, nil
+	}
+	if rc := C.kgpu_preempt_batch(k.h, (*C.int32_t)(unsafe.Pointer(&pods[0])), (*C.int32_t)(unsafe.Pointer(&lvl[0])),
+		C.int64_t(len(keys)), (*C.uint64_t)(unsafe.Pointer(&keys[0])), (*C.uint32_t)(unsafe.Pointer(&victims[0]))); rc != C.KGPU_OK {
+		return nil, nil, k.err("kgpu_preempt_batch")
+	}
+	return keys, victims, nil
+}

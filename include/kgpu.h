@@ -195,6 +195,36 @@ int kgpu_place_batch_ex(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out
  * kgpu_place_batch_ex on the batch with every failed gang deleted.  Members may differ in k and min_mem_mib.
  * gang == NULL is kgpu_place_batch_ex.  Flags, min_mem_mib limits and single-device handles as there. */
 int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, int64_t P, uint64_t *out_keys, int flags);
+/* Preemption (kube-scheduler's PostFilter for GPU pods): for a pod that fits nowhere, the node, GPUs and
+ * lowest-priority running pods to evict.  No reference counterpart (DeviceScheduler has no preemption hook,
+ * gpu_scheduler.go:21-71).  Single-device handles only (KGPU_ERR_STATE otherwise).
+ *
+ * The HOLDER TABLE holds one row of 8 int32 per node (laid out like gpu_mem): for GPU slot i, -1 (the GPU cannot be
+ * evicted) or level << 3 | owner, with level 0..15 the priority level of the running pod that holds the GPU and owner
+ * 0..7 that pod's number on this node.  All GPUs with the same owner on a node belong to one pod, are evicted
+ * together and must carry the same level.  The entry of a free GPU (bit set in free_mask) is ignored.
+ *   kgpu_upload_holders   sets the whole table (n = kgpu_num_nodes rows).
+ *   kgpu_set_holders      replaces n rows (node indices idx[n], rows holders[n][8]) in one copy; a node listed
+ *                         twice gets its LAST row.
+ * An entry that is neither -1 nor 0..127, or an owner with two levels in one row, is KGPU_ERR_INVALID and leaves the
+ * table unchanged.  The table's device memory (32 B per node) is allocated by the first upload.  kgpu_upload_nodes
+ * resets the table to all -1; kgpu_update_node and kgpu_set_free_mask(s) leave it alone, so the caller keeps it in
+ * step with the masks.
+ *
+ * kgpu_preempt_batch: pods[P][4] as for kgpu_score_batch, lvl[P] each pod's level 0..15 (KGPU_ERR_INVALID
+ * otherwise).  For pod p, GPU i of node n is AVAILABLE if it is free, or if its entry is not -1 and its holder's
+ * level is < lvl[p]; either way it must pass min_mem_mib as in scoring.  A candidate is (n, S) with S a k-subset of
+ * available GPUs; its victims V(S) are the owners of the GPUs of S that are not free.  Candidates are ordered by
+ * (max level in V, |V|, cost(S), node id, S), smallest first, an empty V before every non-empty one.
+ *   out_keys[p]     the winner's key in the standard format, or KGPU_NO_FIT (no candidate, or k outside 0..8);
+ *   out_victims[p]  bit o = owner o of the winner's node is evicted; 0 when nothing is.
+ * So a pod that fits without eviction gets exactly its kgpu_score_batch key and victims 0, a level-0 pod never evicts,
+ * and without a holder table the call equals kgpu_score_batch.  Snapshot semantics: nothing is evicted or taken, and
+ * two pods of one batch may name the same victims.  Host buffers, synchronous. */
+int kgpu_upload_holders(kgpu_t *h, const int32_t *holders, int64_t n);
+int kgpu_set_holders(kgpu_t *h, const int64_t *idx, const int32_t *holders, int64_t n);
+int kgpu_preempt_batch(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_t P, uint64_t *out_keys,
+                       uint32_t *out_victims);
 /* Copy the current free masks (n = kgpu_num_nodes entries) back to the host. */
 int kgpu_get_free_masks(kgpu_t *h, int32_t *out_free_mask, int64_t n);
 

@@ -83,6 +83,7 @@ using gpuplugintypes::ResourceGPU;
 const char *const GPUTopologyGeneration = "gpu/gpu-generate-topology";
 const char *const GPUMinMemoryMiB = "gpu/gpu-min-memory-mib";
 const char *const GPUGangID = "gpu/gpu-gang-id";
+const char *const GPUPriorityLevel = "gpu/gpu-priority-level";
 
 namespace {
 
@@ -450,6 +451,7 @@ void NvidiaGPUScheduler::AddNode(const std::string &nodeName, types::NodeInfo *n
             }
     }
     if (fresh) dirty_ = true; else changed_.push_back(nodeName);
+    holdersChanged_.insert(nodeName);
 }
 
 void NvidiaGPUScheduler::RemoveNode(const std::string &nodeName) {              // gpu_scheduler.go:30-32
@@ -458,6 +460,7 @@ void NvidiaGPUScheduler::RemoveNode(const std::string &nodeName) {              
     if (it != nodes_.end()) {
         it->second.removed = true;
         changed_.push_back(nodeName);
+        holdersChanged_.insert(nodeName);
     }
 }
 
@@ -542,6 +545,7 @@ std::string NvidiaGPUScheduler::flushNodes() {
     }
     if (anyMem && kgpu_upload_gpu_memory(handle_, mem.data(), (int64_t)n) != KGPU_OK) return lastError_ = kgpu_last_error(handle_);
     dirty_ = false;
+    holdersReset_ = true;                                // kgpu_upload_nodes reset the holder table
     return "";
 }
 
@@ -562,10 +566,60 @@ int32_t minMemOf(const types::PodInfo &pod) {
     const int64_t need = getOr0(pod.Requests, GPUMinMemoryMiB);
     return (int32_t)std::max<int64_t>(0, std::min<int64_t>(need, std::numeric_limits<int32_t>::max()));
 }
+int levelOf(const types::PodInfo &pod) {
+    return (int)std::max<int64_t>(0, std::min<int64_t>(getOr0(pod.Requests, GPUPriorityLevel), 15));
+}
 }  // namespace
 
+std::string NvidiaGPUScheduler::PreemptBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
+                                             std::vector<std::vector<std::string>> *victims) {
+    return runBatch(pods, out, BatchMode::Preempt, victims);
+}
+
+// Holder rows from the committed placements: on each node the pods holding GPUs, in name order, are owners 0, 1, ...;
+// a GPU gets level << 3 | owner of the pod that holds it, -1 if no committed placement accounts for it.  Pushed for the
+// nodes changed since the last push (kgpu_set_holders), or all of them after a re-upload reset the table.
+std::string NvidiaGPUScheduler::pushHolders() {
+    std::vector<std::string> names;
+    if (holdersReset_) {
+        names = indexToName_;
+    } else {
+        names.assign(holdersChanged_.begin(), holdersChanged_.end());
+    }
+    std::map<std::string, std::vector<std::pair<std::string, const Placement *>>> held;   // node -> (pod, placement)
+    for (const auto &kv : lastPlacement_)                   // std::map: pods in name order
+        if (kv.second.fits && kv.second.committed && kv.second.gpuMask) held[kv.second.nodeName].emplace_back(kv.first, &kv.second);
+    std::vector<int64_t> idx;
+    std::vector<int32_t> rows;
+    for (const std::string &name : names) {
+        auto it = nodes_.find(name);
+        if (it == nodes_.end()) continue;
+        NodeRecord &rec = it->second;
+        int32_t row[8] = {-1, -1, -1, -1, -1, -1, -1, -1};
+        rec.owners.clear();
+        if (!rec.removed) {
+            for (const auto &hp : held[name]) {
+                if (rec.owners.size() == 8) break;
+                const uint32_t mask = hp.second->gpuMask & rec.usedMask;
+                if (!mask) continue;
+                const int32_t o = (int32_t)rec.owners.size();
+                rec.owners.push_back(hp.first);
+                for (int g = 0; g < 8; g++)
+                    if ((mask >> g) & 1u) row[g] = (int32_t)hp.second->level << 3 | o;
+            }
+        }
+        idx.push_back(rec.index);
+        rows.insert(rows.end(), row, row + 8);
+    }
+    if (!idx.empty() && kgpu_set_holders(handle_, idx.data(), rows.data(), (int64_t)idx.size()) != KGPU_OK)
+        return lastError_ = kgpu_last_error(handle_);
+    holdersChanged_.clear();
+    holdersReset_ = false;
+    return "";
+}
+
 std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
-                                         BatchMode mode) {
+                                         BatchMode mode, std::vector<std::vector<std::string>> *victims) {
     std::string err = flushNodes();
     if (!err.empty()) return err;
     const size_t P = pods.size();
@@ -575,7 +629,7 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     std::vector<size_t> order(P);
     std::vector<int32_t> gang;
     for (size_t p = 0; p < P; p++) order[p] = p;
-    if (mode != BatchMode::Snapshot) {
+    if (mode == BatchMode::Sequential || mode == BatchMode::DryRun) {
         std::map<int64_t, int32_t> dense;
         std::vector<std::vector<size_t>> members;
         std::vector<int32_t> gangOf(P, 0);
@@ -618,7 +672,15 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
         req[i * 4 + 3] = minMemOf(*pods[p]);
     }
     std::vector<uint64_t> dev(P, KGPU_NO_FIT);
-    const int rc = mode == BatchMode::Snapshot ? kgpu_score_batch(handle_, req.data(), (int64_t)P, dev.data())
+    std::vector<uint32_t> owners(P, 0);
+    std::vector<int32_t> lvl(P, 0);
+    if (mode == BatchMode::Preempt) {
+        for (size_t i = 0; i < P; i++) lvl[i] = levelOf(*pods[order[i]]);
+        err = pushHolders();
+        if (!err.empty()) return err;
+    }
+    const int rc = mode == BatchMode::Preempt  ? kgpu_preempt_batch(handle_, req.data(), lvl.data(), (int64_t)P, dev.data(), owners.data())
+                   : mode == BatchMode::Snapshot ? kgpu_score_batch(handle_, req.data(), (int64_t)P, dev.data())
                                                : kgpu_place_batch_gang(handle_, req.data(), gang.empty() ? nullptr : gang.data(),
                                                                        (int64_t)P, dev.data(),
                                                                        mode == BatchMode::DryRun ? KGPU_PLACE_DRY_RUN : 0);
@@ -626,9 +688,11 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     std::vector<uint64_t> keys(P, KGPU_NO_FIT);           // back in the caller's order
     for (size_t i = 0; i < P; i++) keys[order[i]] = dev[i];
     out->assign(P, Placement());
+    if (victims) victims->assign(P, {});
     for (size_t p = 0; p < P; p++) {
         Placement &pl = (*out)[p];
         pl.key = keys[p];
+        pl.level = levelOf(*pods[p]);
         if (keys[p] != KGPU_NO_FIT) {
             pl.fits = true;
             pl.cost = KGPU_KEY_COST(keys[p]);
@@ -637,8 +701,15 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
             if (mode == BatchMode::Sequential) {            // the device already took them: TakePodResources is a no-op
                 nodes_[pl.nodeName].usedMask |= pl.gpuMask;
                 pl.committed = true;
+                holdersChanged_.insert(pl.nodeName);
+            }
+            if (mode == BatchMode::Preempt) {                // order == identity: gangs are not reordered here
+                const NodeRecord &rec = nodes_[pl.nodeName];
+                for (int o = 0; o < 8; o++)
+                    if (((owners[p] >> o) & 1u) && (size_t)o < rec.owners.size()) (*victims)[p].push_back(rec.owners[(size_t)o]);
             }
         }
+        if (mode == BatchMode::Preempt) continue;            // a proposal that needs evictions first: not remembered
         if (!pods[p]->Name.empty()) lastPlacement_[pods[p]->Name] = pl;
     }
     return "";
@@ -703,6 +774,7 @@ bool NvidiaGPUScheduler::PodFitsDevice(types::NodeInfo *nodeInfo, types::PodInfo
         pl.cost = nk >> 8;
         pl.gpuMask = nk & 0xFFu;
         pl.nodeName = rec->name;
+        pl.level = levelOf(*podInfo);
         pl.key = ((uint64_t)pl.cost << 40) | ((uint64_t)rec->index << 8) | pl.gpuMask;
         lastPlacement_[podInfo->Name] = pl;
     }
@@ -734,6 +806,7 @@ std::string NvidiaGPUScheduler::PodAllocate(types::NodeInfo *nodeInfo, types::Po
         pl.cost = nk >> 8;
         pl.gpuMask = nk & 0xFFu;
         pl.nodeName = here->name;
+        pl.level = levelOf(*podInfo);
         pl.key = ((uint64_t)pl.cost << 40) | ((uint64_t)here->index << 8) | pl.gpuMask;
         if (!podInfo->Name.empty()) lastPlacement_[podInfo->Name] = pl;
     } else {
@@ -787,6 +860,7 @@ std::string NvidiaGPUScheduler::TakePodResources(types::NodeInfo * /*nodeInfo*/,
         return lastError_ = "TakePodResources: GPUs of pod " + podInfo->Name + " already in use on " + n->first + " (score the pod again)";
     n->second.usedMask |= it->second.gpuMask;
     it->second.committed = true;
+    holdersChanged_.insert(n->first);
     return pushMask(n->second);
 }
 
@@ -800,6 +874,7 @@ std::string NvidiaGPUScheduler::ReturnPodResources(types::NodeInfo * /*nodeInfo*
     }
     n->second.usedMask &= ~it->second.gpuMask;
     lastPlacement_.erase(it);
+    holdersChanged_.insert(n->first);
     return pushMask(n->second);
 }
 

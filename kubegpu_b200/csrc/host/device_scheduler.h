@@ -20,6 +20,7 @@
 #include <cstdint>
 #include <map>
 #include <memory>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -92,6 +93,9 @@ extern const char *const GPUMinMemoryMiB;         // "gpu/gpu-min-memory-mib"
 // distributed training job).  Pods of one PlaceBatch / ProposeBatch call with the same nonzero value are placed all
 // or nothing; 0 or absent = the pod is on its own.
 extern const char *const GPUGangID;               // "gpu/gpu-gang-id"
+// Extension: pod-level request "my priority level", 0..15 (values outside are clamped), default 0.  PreemptBatch lets a
+// pod evict running pods of a LOWER level; every placement records the level of its pod.
+extern const char *const GPUPriorityLevel;        // "gpu/gpu-priority-level"
 
 // ---- gpu.go, function for function ------------------------------------------------
 types::ResourceList TranslateGPUResources(int64_t neededGPUs, const types::ResourceList &nodeResources,
@@ -136,6 +140,7 @@ struct Placement {
     uint32_t gpuMask = 0;       // bit i = GPU slot i of that node
     uint64_t key = UINT64_MAX;  // raw (cost<<40 | node_id<<8 | mask)
     bool committed = false;     // the GPUs are already taken on the device (PlaceBatch) / by TakePodResources
+    int level = 0;              // the pod's GPUPriorityLevel
 };
 
 // ---- gpu_scheduler.go: the DeviceScheduler boundary ------------------------------------
@@ -189,6 +194,15 @@ public:
     // This is the conflict resolution ScoreBatch lacks: its snapshot scores hand every pod of equal k the same GPUs.
     // Gangs as in PlaceBatch.
     std::string ProposeBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out);
+    // Preemption (kube-scheduler's PostFilter): for each pod, the best placement when running pods of a lower
+    // GPUPriorityLevel may be evicted -- fewest and lowest-level victims first (lowest highest victim level, then fewest
+    // victims, then cost, node, GPUs), see kgpu_preempt_batch.  A pod that fits without eviction gets its ScoreBatch
+    // placement and no victims.  (*victims)[p] names the running pods to evict, in name order.  The running pods are the
+    // committed placements (PlaceBatch, TakePodResources) until ReturnPodResources; GPUs in use that no committed
+    // placement accounts for are never evicted.  Snapshot semantics: nothing is evicted, taken or remembered, two pods
+    // may name the same victims, and gang ids are ignored.
+    std::string PreemptBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
+                             std::vector<std::vector<std::string>> *victims);
     std::string LastError() const { return lastError_; }
     const TreeCache &cache() const { return cache_; }
     bool hasDevice() const { return handle_ != nullptr; }
@@ -204,6 +218,7 @@ public:
         uint32_t presentMask = 0, usedMask = 0;
         bool explicitTopo = false;
         bool removed = false;
+        std::vector<std::string> owners;      // holder-table owner o -> pod name, as last pushed to the device
     };
     const NodeRecord *node(const std::string &nodeName) const;
     static int64_t PodGPUCount(const types::PodInfo &podInfo);     // k of gpu.go:295-303
@@ -212,10 +227,12 @@ private:
     std::string syncNode(const NodeRecord &rec);
     std::string flushNodes();
     std::string scoreOne(const NodeRecord &rec, int k, int32_t minMemMiB, uint32_t *nodeKey);
-    enum class BatchMode { Snapshot, Sequential, DryRun };
-    std::string runBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out, BatchMode mode);
+    enum class BatchMode { Snapshot, Sequential, DryRun, Preempt };
+    std::string runBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out, BatchMode mode,
+                         std::vector<std::vector<std::string>> *victims = nullptr);
     const NodeRecord *recordOf(const types::NodeInfo *nodeInfo) const;
     std::string pushMask(NodeRecord &rec);
+    std::string pushHolders();
     TreeCache cache_;
     std::map<std::string, NodeRecord> nodes_;
     std::vector<std::string> indexToName_;
@@ -224,6 +241,8 @@ private:
     kgpu_ctx *handle_ = nullptr;
     bool dirty_ = false;                                // node COUNT changed: the device array must be re-uploaded
     std::vector<std::string> changed_;                  // existing nodes whose matrix / presence changed (kgpu_update_node)
+    std::set<std::string> holdersChanged_;              // nodes whose running pods changed since the last holder push
+    bool holdersReset_ = true;                          // the device table was reset (re-upload): push every row
     bool groupSchedulerMode_ = false;
     std::string lastError_;
 };

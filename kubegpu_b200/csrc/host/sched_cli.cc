@@ -10,13 +10,14 @@
 //   addnode NAME KUBEALLOC [key=val ...]        AddNode with Allocatable = {key: val}
 //   rmnode NAME                                 RemoveNode
 //   topo NAME v0 .. v63                         SetNodeTopology (extension)
-//   pod NAME [topogen=V] [minmem=MiB] [gang=ID] {run|init CNAME req=N [kube=N] [dev:key=val ...]}...
+//   pod NAME [topogen=V] [minmem=MiB] [gang=ID] [priority=L] {run|init CNAME req=N [kube=N] [dev:key=val ...]}...
 //   fits NODE POD                               PodFitsDevice  -> fits/score + rewritten requests
 //   allocate NODE POD                           PodAllocate    -> error text + AllocateFrom
 //   take POD | return POD                       TakePodResources / ReturnPodResources
 //   scorebatch POD...                           ScoreBatch (GPU)
 //   placebatch POD...                           PlaceBatch (GPU, sequential, takes the GPUs)
 //   proposebatch POD...                         ProposeBatch (GPU, sequential on a scratch copy, takes nothing)
+//   preemptbatch POD...                         PreemptBatch (GPU): placements when lower-priority pods may be evicted
 //   addjson NAME FILE [nvml]                    AddNodeFromGpusInfo (node agent JSON), dumps names + matrix
 //   visible POD                                 NVIDIA_VISIBLE_DEVICES per container (node agent Allocate)
 //   cache                                       dump the tree cache
@@ -144,6 +145,8 @@ int main(int argc, char **argv) {
                     pod.Requests[GPUMinMemoryMiB] = atoll(tok.c_str() + 7);
                 } else if (tok.compare(0, 5, "gang=") == 0) {
                     pod.Requests[GPUGangID] = atoll(tok.c_str() + 5);
+                } else if (tok.compare(0, 9, "priority=") == 0) {
+                    pod.Requests[GPUPriorityLevel] = atoll(tok.c_str() + 9);
                 } else if (cur && tok.compare(0, 4, "req=") == 0) {
                     cur->Requests[gpuplugintypes::ResourceGPU] = atoll(tok.c_str() + 4);
                 } else if (cur && tok.compare(0, 5, "kube=") == 0) {
@@ -188,6 +191,20 @@ int main(int argc, char **argv) {
             for (size_t i = 0; i < out.size(); i++)
                 printf("  %s fits=%d cost=%u node=%s mask=0x%02x\n", pods[i]->Name.c_str(), out[i].fits ? 1 : 0, out[i].cost,
                        out[i].nodeName.c_str(), out[i].gpuMask);
+        } else if (cmd == "preemptbatch") {
+            std::vector<const types::PodInfo *> pods;
+            std::string podName;
+            while (in >> podName)
+                if (g_pods.count(podName)) pods.push_back(&g_pods[podName]);
+            std::vector<Placement> out;
+            std::vector<std::vector<std::string>> victims;
+            printf("  err=%s\n", sched.PreemptBatch(pods, &out, &victims).c_str());
+            for (size_t i = 0; i < out.size(); i++) {
+                std::string names;
+                for (const std::string &v : victims[i]) names += (names.empty() ? "" : ",") + v;
+                printf("  %s fits=%d cost=%u node=%s mask=0x%02x victims=%s\n", pods[i]->Name.c_str(), out[i].fits ? 1 : 0,
+                       out[i].cost, out[i].nodeName.c_str(), out[i].gpuMask, names.c_str());
+            }
         } else if (cmd == "cache") {
             // sorted by (tree text) so the transcript does not depend on insertion order
             std::vector<std::string> rows;

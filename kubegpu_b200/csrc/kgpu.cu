@@ -17,6 +17,7 @@
 
 #include "multi_device.h"
 #include "place_sequential.cuh"
+#include "preempt.cuh"
 #include "sparse_work.h"
 #include "peer_exchange.cuh"
 #include "score_pairs.cuh"
@@ -67,6 +68,15 @@ struct kgpu_shard {
     uint32_t *d_qout = nullptr;
     int64_t query_cap = 0;
     int32_t *d_free_scratch = nullptr;   // kgpu_place_batch_ex(KGPU_PLACE_DRY_RUN): the masks the dry run consumes
+    int32_t *d_hold = nullptr;       // [n][8] holder table (kgpu_upload_holders / kgpu_set_holders), allocated on first upload
+    int64_t hold_cap = 0;
+    bool has_hold = false;           // false = every entry is -1 (no upload since the last kgpu_upload_nodes)
+    int32_t *d_lvl = nullptr;        // kgpu_preempt_batch scratch [pre_cap]: pod levels, compacted pod positions,
+    int32_t *d_pidx = nullptr;       //   their preemption keys, victims, and the compacted count
+    unsigned long long *d_pkey = nullptr;
+    uint32_t *d_victims = nullptr;
+    int *d_pcnt = nullptr;
+    int64_t pre_cap = 0;
     int64_t free_scratch_cap = 0;
     int64_t class_count[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     int64_t n_slots = 0, slot_cap = 0;
@@ -524,6 +534,12 @@ void free_shard(kgpu_shard &s) {
     if (s.d_fit) cudaFree(s.d_fit);
     if (s.h_fit) cudaFreeHost(s.h_fit);
     if (s.d_free_scratch) cudaFree(s.d_free_scratch);
+    if (s.d_hold) cudaFree(s.d_hold);
+    if (s.d_lvl) cudaFree(s.d_lvl);
+    if (s.d_pidx) cudaFree(s.d_pidx);
+    if (s.d_pkey) cudaFree(s.d_pkey);
+    if (s.d_victims) cudaFree(s.d_victims);
+    if (s.d_pcnt) cudaFree(s.d_pcnt);
     if (s.d_query) cudaFree(s.d_query);
     if (s.d_qout) cudaFree(s.d_qout);
     if (s.d_pods) cudaFree(s.d_pods);
@@ -687,7 +703,9 @@ int kgpu_upload_nodes(kgpu_t *h, const int32_t *topo, const int32_t *free_mask, 
             if (s.d_free) cudaFree(s.d_free);
             if (s.d_mem) cudaFree(s.d_mem);
             if (s.d_slot_of) cudaFree(s.d_slot_of);
+            if (s.d_hold) cudaFree(s.d_hold);
             s.d_topo = nullptr; s.d_free = nullptr; s.d_mem = nullptr; s.d_slot_of = nullptr; s.cap = 0; s.n = 0;
+            s.d_hold = nullptr; s.hold_cap = 0;
             KGPU_UP(cudaMalloc(&s.d_topo, (size_t)cnt * 256));
             KGPU_UP(cudaMalloc(&s.d_free, (size_t)cnt * 4));
             KGPU_UP(cudaMalloc(&s.d_mem, (size_t)cnt * 32));
@@ -707,6 +725,7 @@ int kgpu_upload_nodes(kgpu_t *h, const int32_t *topo, const int32_t *free_mask, 
             KGPU_UP(cudaGetLastError());
         }
         s.n = cnt;
+        s.has_hold = false;            // a new node array has no holders
         s.node_id_base = node_id_base + off;
         s.order_dirty = true;
         s.compact_dirty = true;
@@ -991,6 +1010,170 @@ int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, i
         KGPU_CUDA(h, cudaEventElapsedTime(&ms, s.ev0, s.ev1));
         h->last_kernel_ms = ms;
     }
+    return KGPU_OK;
+}
+
+namespace {
+// Holder rows: every entry -1 or level << 3 | owner (level 0..15, owner 0..7), one level per owner within a row.
+int validate_holders(kgpu_ctx *h, const char *fn, const int32_t *rows, int64_t n) {
+    for (int64_t r = 0; r < n; r++) {
+        int32_t level_of[8] = {-1, -1, -1, -1, -1, -1, -1, -1};
+        for (int g = 0; g < 8; g++) {
+            const int32_t e = rows[r * 8 + g];
+            if (e == -1) continue;
+            if (e < 0 || e > 127)
+                return fail(h, KGPU_ERR_INVALID, "%s: row %lld GPU %d: entry %d is neither -1 nor level << 3 | owner with level 0..15",
+                            fn, (long long)r, g, e);
+            const int32_t o = e & 7, lv = e >> 3;
+            if (level_of[o] >= 0 && level_of[o] != lv)
+                return fail(h, KGPU_ERR_INVALID, "%s: row %lld: owner %d has levels %d and %d", fn, (long long)r, o, level_of[o], lv);
+            level_of[o] = lv;
+        }
+    }
+    return KGPU_OK;
+}
+
+// The holder table of shard s exists on the device (first use: allocated and set to all -1).
+int ensure_holders(kgpu_ctx *h, kgpu_shard &s) {
+    KGPU_CUDA(h, cudaSetDevice(s.dev));
+    if (s.hold_cap < s.n) {
+        if (s.d_hold) cudaFree(s.d_hold);
+        s.d_hold = nullptr; s.hold_cap = 0; s.has_hold = false;
+        KGPU_CUDA(h, cudaMalloc(&s.d_hold, (size_t)s.n * 32));
+        s.hold_cap = s.n;
+    }
+    if (!s.has_hold && s.n > 0) KGPU_CUDA(h, cudaMemsetAsync(s.d_hold, 0xFF, (size_t)s.n * 32, s.stream));
+    s.has_hold = true;
+    return KGPU_OK;
+}
+
+int ensure_preempt_capacity(kgpu_ctx *h, kgpu_shard &s, int64_t P) {
+    if (P <= s.pre_cap) return KGPU_OK;
+    const int64_t cap = std::max<int64_t>(1024, P + P / 4);
+    KGPU_CUDA(h, cudaSetDevice(s.dev));
+    if (s.d_lvl) cudaFree(s.d_lvl);
+    if (s.d_pidx) cudaFree(s.d_pidx);
+    if (s.d_pkey) cudaFree(s.d_pkey);
+    if (s.d_victims) cudaFree(s.d_victims);
+    s.d_lvl = nullptr; s.d_pidx = nullptr; s.d_pkey = nullptr; s.d_victims = nullptr; s.pre_cap = 0;
+    if (!s.d_pcnt) KGPU_CUDA(h, cudaMalloc(&s.d_pcnt, sizeof(int)));
+    KGPU_CUDA(h, cudaMalloc(&s.d_lvl, (size_t)cap * 4));
+    KGPU_CUDA(h, cudaMalloc(&s.d_pidx, (size_t)cap * 4));
+    KGPU_CUDA(h, cudaMalloc(&s.d_pkey, (size_t)cap * 8));
+    KGPU_CUDA(h, cudaMalloc(&s.d_victims, (size_t)cap * 4));
+    s.pre_cap = cap;
+    return KGPU_OK;
+}
+}  // namespace
+
+int kgpu_upload_holders(kgpu_t *h, const int32_t *holders, int64_t n) {
+    if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_holders: NULL handle");
+    std::lock_guard<std::mutex> g(h->mu);
+    if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_upload_holders: needs a single-device handle");
+    if (n != h->n_total || (n > 0 && !holders)) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_holders: n must equal kgpu_num_nodes");
+    int rc = validate_holders(h, "kgpu_upload_holders", holders, n);
+    if (rc != KGPU_OK) return rc;
+    kgpu_shard &s = h->shards[0];
+    rc = ensure_holders(h, s);
+    if (rc != KGPU_OK) return rc;
+    if (n > 0) KGPU_CUDA(h, cudaMemcpyAsync(s.d_hold, holders, (size_t)n * 32, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, cudaStreamSynchronize(s.stream));
+    return KGPU_OK;
+}
+
+int kgpu_set_holders(kgpu_t *h, const int64_t *idx, const int32_t *holders, int64_t n) {
+    if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_set_holders: NULL handle");
+    std::lock_guard<std::mutex> g(h->mu);
+    if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_set_holders: needs a single-device handle");
+    if (n < 0 || (n > 0 && (!idx || !holders))) return fail(h, KGPU_ERR_INVALID, "kgpu_set_holders: bad arguments");
+    for (int64_t i = 0; i < n; i++)
+        if (idx[i] < 0 || idx[i] >= h->n_total)
+            return fail(h, KGPU_ERR_INVALID, "kgpu_set_holders: index %lld out of range", (long long)idx[i]);
+    int rc = validate_holders(h, "kgpu_set_holders", holders, n);
+    if (rc != KGPU_OK || n == 0) return rc;
+    // the LAST row wins when a node is listed more than once; one staging buffer: [m] local indices | [m][8] rows
+    std::vector<std::pair<int64_t, int64_t>> ent((size_t)n);
+    for (int64_t i = 0; i < n; i++) ent[(size_t)i] = {idx[i], i};
+    std::sort(ent.begin(), ent.end());
+    std::vector<int64_t> pick;
+    for (size_t e = 0; e < ent.size(); e++)
+        if (e + 1 == ent.size() || ent[e + 1].first != ent[e].first) pick.push_back(ent[e].second);
+    const int64_t m = (int64_t)pick.size();
+    const int64_t rows_off = (m + 3) / 4 * 4;        // rows start 16-byte aligned
+    std::vector<int32_t> stage((size_t)(rows_off + m * 8));
+    for (int64_t j = 0; j < m; j++) {
+        stage[(size_t)j] = (int32_t)idx[pick[(size_t)j]];
+        memcpy(&stage[(size_t)(rows_off + j * 8)], holders + pick[(size_t)j] * 8, 32);
+    }
+    kgpu_shard &s = h->shards[0];
+    rc = ensure_holders(h, s);
+    if (rc != KGPU_OK) return rc;
+    rc = ensure_upd_capacity(h, s, (int64_t)stage.size() / 2 + 1);   // d_upd holds 2 * upd_cap int32
+    if (rc != KGPU_OK) return rc;
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_upd, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, s.stream));
+    kgpu::scatter_holders<<<(unsigned)((m + 255) / 256), 256, 0, s.stream>>>(
+        s.d_upd, reinterpret_cast<const int4 *>(s.d_upd + rows_off), m, reinterpret_cast<int4 *>(s.d_hold));
+    h->launches++;
+    KGPU_CUDA(h, cudaGetLastError());
+    KGPU_CUDA(h, cudaStreamSynchronize(s.stream));
+    return KGPU_OK;
+}
+
+int kgpu_preempt_batch(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_t P, uint64_t *out_keys,
+                       uint32_t *out_victims) {
+    if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_batch: NULL handle");
+    std::lock_guard<std::mutex> g(h->mu);
+    if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_preempt_batch: needs a single-device handle");
+    if (P < 0 || (P > 0 && (!pods || !lvl || !out_keys || !out_victims)))
+        return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_batch: bad arguments");
+    for (int64_t p = 0; p < P; p++)
+        if (lvl[p] < 0 || lvl[p] > 15) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_batch: lvl[%lld] = %d outside 0..15", (long long)p, lvl[p]);
+    if (P == 0) return KGPU_OK;
+    if (P > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_batch: more than 2^31 pods");
+    kgpu_shard &s = h->shards[0];
+    int rc = ensure_pod_capacity(h, s, P);
+    if (rc == KGPU_OK) rc = ensure_preempt_capacity(h, s, P);
+    if (rc != KGPU_OK) return rc;
+    int has_mem = 0;
+    for (int64_t p = 0; p < P && !has_mem; p++) has_mem = pods[4 * p + 3] > 0;
+    KGPU_CUDA(h, cudaSetDevice(s.dev));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_pods, pods, (size_t)P * 16, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, cudaMemsetAsync(s.d_victims, 0, (size_t)P * 4, s.stream));
+    KGPU_CUDA(h, cudaEventRecord(s.ev0, s.stream));
+    // 1. the scoring path, unchanged: every pod that fits without eviction keeps its key (victims 0)
+    rc = launch_score(h, s, s.d_pods, P, s.d_keys, s.stream, has_mem);
+    if (rc != KGPU_OK) return rc;
+    if (s.has_hold && s.n > 0) {
+        // 2. the NO_FIT pods that may evict, compacted on the device; 3. K4 over them only
+        const int4 *pods4 = reinterpret_cast<const int4 *>(s.d_pods);
+        KGPU_CUDA(h, cudaMemcpyAsync(s.d_lvl, lvl, (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
+        KGPU_CUDA(h, cudaMemsetAsync(s.d_pcnt, 0, sizeof(int), s.stream));
+        KGPU_CUDA(h, cudaMemsetAsync(s.d_pkey, 0xFF, (size_t)P * 8, s.stream));
+        const unsigned pb = (unsigned)((P + 255) / 256);
+        kgpu::preempt_compact<<<pb, 256, 0, s.stream>>>(pods4, s.d_lvl, s.d_keys, P, s.d_pidx, s.d_pcnt);
+        kgpu::Weights W;
+        memcpy(W.w, h->W, sizeof W.w);
+        // the compacted count stays on the device: size the grid from P (blocks beyond the count exit at once) for
+        // about 8 waves of resident blocks
+        const int64_t tiles = (s.n + kgpu::PRE_THREADS - 1) / kgpu::PRE_THREADS;
+        if (tiles > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_batch: too many nodes for one launch");
+        int64_t splits = std::max<int64_t>(1, (8 * (int64_t)s.sm_count * 4 + tiles - 1) / tiles);
+        splits = std::min<int64_t>({splits, (P + kgpu::PRE_CHUNK - 1) / kgpu::PRE_CHUNK, 65535});
+        kgpu::preempt_lane_per_node<<<dim3((unsigned)tiles, (unsigned)splits), kgpu::PRE_THREADS, 0, s.stream>>>(
+            reinterpret_cast<const int4 *>(s.d_topo), s.d_free, reinterpret_cast<const int4 *>(s.d_mem),
+            reinterpret_cast<const int4 *>(s.d_hold), s.n, pods4, s.d_lvl, s.d_pidx, s.d_pcnt, W, PC, s.d_pkey);
+        kgpu::preempt_finalize<<<pb, 256, 0, s.stream>>>(s.d_pkey, s.d_pidx, s.d_pcnt, s.d_free, s.d_hold, s.node_id_base,
+                                                         s.d_keys, s.d_victims);
+        h->launches += 3;
+        KGPU_CUDA(h, cudaGetLastError());
+    }
+    KGPU_CUDA(h, cudaEventRecord(s.ev1, s.stream));
+    KGPU_CUDA(h, cudaMemcpyAsync(out_keys, s.d_keys, (size_t)P * 8, cudaMemcpyDeviceToHost, s.stream));
+    KGPU_CUDA(h, cudaMemcpyAsync(out_victims, s.d_victims, (size_t)P * 4, cudaMemcpyDeviceToHost, s.stream));
+    KGPU_CUDA(h, cudaStreamSynchronize(s.stream));
+    float ms = 0.f;
+    KGPU_CUDA(h, cudaEventElapsedTime(&ms, s.ev0, s.ev1));
+    h->last_kernel_ms = ms;
     return KGPU_OK;
 }
 

@@ -166,6 +166,38 @@ class Scorer:
         self._check(self._L.kgpu_place_batch_gang(self._h, pods.ctypes.data, gang.ctypes.data, P, out.ctypes.data, flags))
         return out
 
+    # -- preemption (PostFilter) -----------------------------------------------------
+    def upload_holders(self, holders) -> None:
+        """holders[N,8]: per GPU slot -1 (not evictable) or level << 3 | owner (level 0..15, owner 0..7); GPUs of one
+        owner belong to one running pod and carry one level.  Entries of free GPUs are ignored."""
+        hold = _i32(holders)
+        if hold.size != 8 * self.num_nodes:
+            raise ValueError("holders must be [N,8]")
+        self._check(self._L.kgpu_upload_holders(self._h, hold.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), self.num_nodes))
+
+    def set_holders(self, idx, holders) -> None:
+        """Replace the holder rows of nodes idx (one copy); the last row wins on duplicates."""
+        idx = np.ascontiguousarray(idx, dtype=np.int64)
+        hold = _i32(holders)
+        if hold.size != 8 * idx.shape[0]:
+            raise ValueError("holders must be [len(idx),8]")
+        self._check(self._L.kgpu_set_holders(self._h, idx.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
+                                             hold.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), idx.shape[0]))
+
+    def preempt_batch(self, pods, lvl):
+        """(keys uint64[P], victims uint32[P]): for each pod the best placement when running pods of a lower level
+        (lvl[p], 0..15) may be evicted, smallest (max victim level, victim count, cost, node, mask) first.  A pod that
+        fits without eviction gets its score_batch key and victims 0; victims bit o = owner o of the key's node."""
+        pods, lvl = _i32(pods), _i32(lvl)
+        P = pods.size // 4
+        if lvl.size != P:
+            raise ValueError("lvl must hold one level per pod")
+        keys = np.empty(P, dtype=np.uint64)
+        victims = np.empty(P, dtype=np.uint32)
+        self._check(self._L.kgpu_preempt_batch(self._h, pods.ctypes.data, lvl.ctypes.data, P, keys.ctypes.data,
+                                               victims.ctypes.data))
+        return keys, victims
+
     def get_free_masks(self) -> np.ndarray:
         out = np.empty(self.num_nodes, dtype=np.int32)
         self._check(self._L.kgpu_get_free_masks(self._h, out.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), out.shape[0]))

@@ -154,6 +154,40 @@ def gen_c6(N: int = 100_000, P: int = 10_000, seed: int = SEED_C6, node_start: i
     return topo, free, mem, pods
 
 
+SEED_PREEMPT = 0xB2000008
+
+
+def gen_preempt(N: int = 100_000, P: int = 10_000, seed: int = SEED_PREEMPT):
+    """An almost full cluster for preemption: C2's node shapes, each node packed from slot 0 with running pods of 1, 2,
+    4 or 8 GPUs (aligned blocks, the size uniform over those that fit at the position) at priority levels 0..3.  At most
+    one block of 1 or 2 GPUs per node is left free (a quarter of the small blocks are, until one is), so no node has
+    more than 2 free GPUs.  The pending pods are C2's (k uniform over {1, 2, 4, 8}) with levels uniform over 0..4: every
+    k = 4 or 8 pod fits nowhere without eviction.
+    Returns (topo, free, holders[N][8], pods, lvl[P]); holders as kgpu_upload_holders takes them."""
+    topo, _, pods = gen_c2(N, P, seed)
+    hold = np.full((N, 8), -1, dtype=np.int32)
+    free = np.zeros(N, dtype=np.int32)
+    pos = np.zeros(N, dtype=np.int64)
+    owner = np.zeros(N, dtype=np.int64)
+    has_free = np.zeros(N, dtype=bool)
+    for step in range(8):
+        live = pos < 8
+        align = np.where(pos == 0, 8, pos & -pos)
+        size = np.minimum(1 << rand_below(seed, 30 + step, N, 4), align)
+        empty = live & (size <= 2) & ~has_free & (rand_below(seed, 40 + step, N, 4) == 0)
+        held = live & ~empty
+        entry = (rand_below(seed, 50 + step, N, 4) << 3) | owner
+        for g in range(8):
+            blk = (g >= pos) & (g < pos + size)
+            hold[blk & held, g] = entry[blk & held]
+            free |= np.where(blk & empty, 1 << g, 0).astype(np.int32)
+        has_free |= empty
+        owner += held
+        pos = np.where(live, pos + size, pos)
+    lvl = rand_below(seed, 24, P, 5).astype(np.int32)
+    return topo, free, hold, pods, lvl
+
+
 def gen_gangs(N: int = 100_000, P: int = 10_000, seed: int = SEED_GANGS, gang_start: float = 0.1):
     """C2's cluster and pod stream, with distributed training jobs mixed in: at each pod that is not yet in a gang,
     a gang starts with probability ``gang_start`` (default: about a third of the pods end up in gangs).  A gang has
