@@ -61,25 +61,31 @@ __device__ __forceinline__ uint32_t node_key_kf(const PairCosts &C, const PipeCo
     return best_kf<(K < 2 ? 2 : K), (F < 2 ? 2 : F)>(C, pc);
 }
 
-// Per-warp pod table of a chunk, in BUCKET order (pods grouped by k): the per-pod multiplier the
-// enumeration runs on (see score_pairs.cuh: it makes every instruction of the enumeration depend on
-// per-pod data) next to the slot the warp's result for that pod goes to.  Pods sit in groups of
-// SP_GROUP; a bucket loop handles one group per trip: one LDS of the multipliers, the enumerations, one
-// STS of the results, loop control once.  Buckets are padded to whole groups with dummy pods
-// (multiplier 1, result never read: sIdx marks them).
-#ifndef KGPU_SP_GROUP
-#define KGPU_SP_GROUP 2          // pods per trip of a bucket loop: 1, 2 or 4
-#endif
-constexpr int SP_GROUP = KGPU_SP_GROUP;
-static_assert(SP_GROUP == 1 || SP_GROUP == 2 || SP_GROUP == 4, "KGPU_SP_GROUP must be 1, 2 or 4");
-constexpr int SP_POS = SP_CHUNK + 10 * (SP_GROUP - 1);          // positions of a chunk in bucket order, dummies included
-constexpr int SP_TAB = (SP_POS + SP_GROUP - 1) / SP_GROUP + 1;  // groups (+1: the prefetch build reads one past the last)
+// Pod table of a chunk, in BUCKET order (pods grouped by k): the per-pod multiplier the enumeration runs
+// on (see score_pairs.cuh: it makes every instruction of the enumeration depend on per-pod data), one
+// array read by every warp, and one row per warp for the warp's result per pod.  Each bucket starts at a
+// multiple of 4 positions and is padded to one with dummy pods (multiplier 1, result never read: sIdx
+// marks them).  A bucket loop handles sp_width(K, F) pods per trip: one LDS of their multipliers, the
+// enumerations, one STS of the results, loop control once.
+constexpr int SP_PAD = 4;            // bucket alignment in positions: the widest trip
 constexpr uint16_t SP_DUMMY = 0xFFFFu;
 constexpr int SP_MEM_SUB = 4;        // MEM launch: pods of one k are sub-bucketed by a hash of min_mem, so equal requirements sit together
-struct alignas(8 * KGPU_SP_GROUP) SpEnt {
-    uint32_t one[SP_GROUP];     // MEM: the pods' min_mem instead (the MEM loops derive `one` from K)
-    uint32_t best[SP_GROUP];    // warp key of the best (node, subset) of this warp for the pod, INF32 = none
+// positions of a chunk of CH pods (nine padded buckets, then the pods not for this launch), rounded to whole
+// trips, plus one trip: the prefetch build reads one past a bucket's end
+__host__ __device__ constexpr int sp_tab_len(int CH) { return (CH + 9 * (SP_PAD - 1) + SP_PAD - 1) / SP_PAD * SP_PAD + SP_PAD; }
+template <int N>
+struct alignas(16) SpTab {
+    uint32_t one[N];                 // MEM: the pods' min_mem instead (the MEM loops derive `one` from K)
+    uint32_t best[SP_WARPS][N];      // warp key of the best (node, subset) of this warp for the pod, INF32 = none
 };
+static_assert(sp_tab_len(SP_CHUNK) % 4 == 0, "rows of the pod table must stay 16-byte aligned");
+
+// Pods per trip of the (K, F) bucket loop.  Four share the multiplier load, the result store and the loop
+// control; two where four pods' enumerations in flight push values into local memory (cuobjdump -sass).  The
+// MEM loops also hold the penalised copy of the pair costs, which (4, 8) does not fit beside four pods.
+__host__ __device__ constexpr int sp_width(int K, int F, bool MEM) {
+    return (K == 3 && F >= 7) || ((K == 5 || K == 6) && F == 8) || (MEM && K == 4 && F == 8) ? 2 : 4;
+}
 
 // Warp key.  BYTE_KEYS (every cost < 2^16, i.e. every weight <= 2340): cost<<16 | lane<<8 | S, built
 // from the lane key (cost<<8 | S) with ONE PRMT whose selector also encodes "this lane cannot serve
@@ -103,24 +109,27 @@ __device__ __forceinline__ uint32_t sp_warp_key(uint32_t key, const SpFmt f, uin
 }
 
 #ifndef KGPU_SP_PREFETCH
-#define KGPU_SP_PREFETCH 0       // 1: load the next group's multipliers one trip ahead (reads one group past a bucket's end)
+#define KGPU_SP_PREFETCH 0       // 1: load the next trip's multipliers one trip ahead (reads one trip past a bucket's end)
 #endif
-__device__ __forceinline__ void sp_load_ones(const SpEnt *ent, uint32_t (&ones)[SP_GROUP]) {
-    if (SP_GROUP == 4) {
-        const uint4 o = *reinterpret_cast<const uint4 *>(ent->one);          // one LDS.128
-        ones[0] = o.x; ones[1 % SP_GROUP] = o.y; ones[2 % SP_GROUP] = o.z; ones[3 % SP_GROUP] = o.w;
-    } else if (SP_GROUP == 2) {
-        const uint2 o = *reinterpret_cast<const uint2 *>(ent->one);          // one LDS.64
-        ones[0] = o.x; ones[1 % SP_GROUP] = o.y;
+template <int W>
+__device__ __forceinline__ void sp_load_ones(const uint32_t *p, uint32_t (&ones)[W]) {
+    static_assert(W == 2 || W == 4, "a trip is 2 or 4 pods");
+    if (W == 4) {
+        const uint4 o = *reinterpret_cast<const uint4 *>(p);                 // one LDS.128
+        ones[0] = o.x; ones[1] = o.y; ones[2 % W] = o.z; ones[3 % W] = o.w;
     } else {
-        ones[0] = ent->one[0];
+        const uint2 o = *reinterpret_cast<const uint2 *>(p);                 // one LDS.64
+        ones[0] = o.x; ones[1] = o.y;
     }
 }
 
-// One (K, F) loop: all pods of the chunk that want K GPUs, enumerating positions 0..F-1.
+// One (K, F) loop: all pods of the chunk that want K GPUs, enumerating positions 0..F-1.  one: the chunk's
+// multipliers, best: this warp's result row, both indexed by bucket-order position.
 template <int K, int F, bool PER_PAIR, bool MEM, bool BYTE_KEYS>
 __device__ __forceinline__ void sp_bucket(const PairCosts &C, const PipeConsts pc, uint32_t nfree, bool valid,
-                                          const int32_t (&mem)[8], uint32_t lane_field, SpEnt *tab, int begin, int end) {
+                                          const int32_t (&mem)[8], uint32_t lane_field, const uint32_t *one,
+                                          uint32_t *best, int begin, int end) {
+    constexpr int W = sp_width(K, F, MEM);
     // (begin >> 30) is 0; tying the test to this chunk's bucket offset keeps the compiler from hoisting the
     // nine per-K selectors to the top of the kernel, where they cost nine registers for the whole run.
     const uint32_t need_free = (uint32_t)K + ((uint32_t)begin >> 30);
@@ -130,24 +139,24 @@ __device__ __forceinline__ void sp_bucket(const PairCosts &C, const PipeConsts p
     uint32_t elig = 0;
     PairCosts C2 = C;
 #if KGPU_SP_PREFETCH
-    uint32_t nxt[SP_GROUP];
-    sp_load_ones(reinterpret_cast<SpEnt *>(reinterpret_cast<char *>(tab) + (uint32_t)begin * 8u), nxt);
+    uint32_t nxt[W];
+    sp_load_ones<W>(one + begin, nxt);
 #endif
     KGPU_UNROLL((sp_unroll(K, F)))
-    // byte offsets (8 bytes per position, begin and end are whole groups): uniform, because begin and end
-    // come from shared memory, so the loop runs on the uniform datapath and the group address is tab + offset
-    for (uint32_t off = (uint32_t)begin * 8u; off != (uint32_t)end * 8u; off += (uint32_t)sizeof(SpEnt)) {
-        SpEnt *const ent = reinterpret_cast<SpEnt *>(reinterpret_cast<char *>(tab) + off);
-        uint32_t ones[SP_GROUP], v[SP_GROUP];
+    // byte offsets (4 bytes per position, begin and end are multiples of SP_PAD): uniform, because begin and end
+    // come from shared memory, so the loop runs on the uniform datapath and both addresses are base + offset
+    for (uint32_t off = (uint32_t)begin * 4u; off != (uint32_t)end * 4u; off += 4u * W) {
+        const uint32_t *const op = reinterpret_cast<const uint32_t *>(reinterpret_cast<const char *>(one) + off);
+        uint32_t ones[W], v[W];
 #if KGPU_SP_PREFETCH
 #pragma unroll
-        for (int g = 0; g < SP_GROUP; g++) ones[g] = nxt[g];
-        sp_load_ones(ent + 1, nxt);                // next trip's multipliers: their LDS latency overlaps this trip
+        for (int g = 0; g < W; g++) ones[g] = nxt[g];
+        sp_load_ones<W>(op + W, nxt);              // next trip's multipliers: their LDS latency overlaps this trip
 #else
-        sp_load_ones(ent, ones);
+        sp_load_ones<W>(op, ones);
 #endif
 #pragma unroll
-        for (int g = 0; g < SP_GROUP; g++) {
+        for (int g = 0; g < W; g++) {
             PipeConsts pcl = pc;
             if (MEM) {
                 const int32_t need = (int32_t)ones[g];
@@ -178,27 +187,33 @@ __device__ __forceinline__ void sp_bucket(const PairCosts &C, const PipeConsts p
                 v[g] = sp_warp_key<BYTE_KEYS>(key, fmt, thirty_two);
             }
         }
-        uint32_t m[SP_GROUP];
+        uint32_t m[W];
 #pragma unroll
-        for (int g = 0; g < SP_GROUP; g++) m[g] = __reduce_min_sync(0xFFFFFFFFu, v[g]);
+        for (int g = 0; g < W; g++) m[g] = __reduce_min_sync(0xFFFFFFFFu, v[g]);
         if (lane_field == 0) {
-            if (SP_GROUP == 4) *reinterpret_cast<uint4 *>(ent->best) = make_uint4(m[0], m[1 % SP_GROUP], m[2 % SP_GROUP], m[3 % SP_GROUP]);
-            else if (SP_GROUP == 2) *reinterpret_cast<uint2 *>(ent->best) = make_uint2(m[0], m[1 % SP_GROUP]);   // one STS.64
-            else ent->best[0] = m[0];
+            void *const bp = reinterpret_cast<char *>(best) + off;
+            if (W == 4) *reinterpret_cast<uint4 *>(bp) = make_uint4(m[0], m[1], m[2 % W], m[3 % W]);   // one STS.128
+            else *reinterpret_cast<uint2 *>(bp) = make_uint2(m[0], m[1]);                              // one STS.64
         }
     }
 }
 
 template <int K, bool PER_PAIR, bool MEM, bool BYTE_KEYS>
 __device__ __forceinline__ void sp_run_k(int F, const PairCosts &C, const PipeConsts pc, uint32_t nfree, bool valid,
-                                         const int32_t (&mem)[8], uint32_t lane_field, SpEnt *tab, int begin, int end) {
-    if (begin >= end || F < K) return;             // F < K: no lane of this warp has K free GPUs
+                                         const int32_t (&mem)[8], uint32_t lane_field, const uint32_t *one,
+                                         uint32_t *best, int begin, int end) {
+    if (begin >= end) return;
+    if (F < K) {                                   // no lane of this warp has K free GPUs: no result for these pods
+        for (int q = begin / 4 + (int)(lane_field >> 8); q < end / 4; q += 32)
+            reinterpret_cast<uint4 *>(best)[q] = make_uint4(INF32, INF32, INF32, INF32);
+        return;
+    }
 #define KGPU_SP_CASE(FF)                                                                                         \
     case FF:                                                                                                     \
-        if (FF >= K) sp_bucket<K, (FF >= K ? FF : K), PER_PAIR, MEM, BYTE_KEYS>(C, pc, nfree, valid, mem, lane_field, tab, begin, end); \
+        if (FF >= K) sp_bucket<K, (FF >= K ? FF : K), PER_PAIR, MEM, BYTE_KEYS>(C, pc, nfree, valid, mem, lane_field, one, best, begin, end); \
         break;
     if (K <= 1) {                                  // F does not matter for k = 0, 1
-        sp_bucket<K, 8, PER_PAIR, MEM, BYTE_KEYS>(C, pc, nfree, valid, mem, lane_field, tab, begin, end);
+        sp_bucket<K, 8, PER_PAIR, MEM, BYTE_KEYS>(C, pc, nfree, valid, mem, lane_field, one, best, begin, end);
         return;
     }
     switch (F) {
@@ -383,11 +398,11 @@ score_pairs_sparse(const int4 *__restrict__ rec, const uint32_t *__restrict__ me
     static_assert(!TMA || (STREAM && !MEM), "the TMA instantiation is a streaming one");
     constexpr int SUB = MEM ? SP_MEM_SUB : 1, NB = 9 * SUB + 1;     // sort buckets: (k, sub) for k = 0..8, then "not for this launch"
     constexpr int CH = TMA ? SP_TMA_PODS : SP_CHUNK;                // pods per chunk of the block's pod sort
-    constexpr int POS = CH + 10 * (SP_GROUP - 1), TAB = (POS + SP_GROUP - 1) / SP_GROUP + 1;
-    __shared__ int32_t sCnt[NB], sOff[12], sPad[9];  // sOff[11]: bit k set = bucket k has pods (STREAM builds test it per tile)
-    __shared__ uint8_t sK[CH];
+    constexpr int POS = sp_tab_len(CH);                // bucket-order positions
+    constexpr int PPT = (CH + SP_THREADS - 1) / SP_THREADS;         // pods per thread in the pod sort
+    __shared__ int32_t sCnt[NB], sOff[12];             // sOff[11]: bit k set = bucket k has pods (STREAM builds test it per tile)
     __shared__ uint16_t sIdx[POS];                     // bucket-order position -> chunk position (SP_DUMMY: padding)
-    __shared__ SpEnt sTab[SP_WARPS][TAB];              // per warp, bucket order: multipliers | results
+    __shared__ SpTab<POS> sTab;                        // bucket order: multipliers | per-warp results
     // position g -> byte (1 << GPU index), g = 0..3 | 4..7.  STREAM builds (few pods per tile) keep the slot's
     // permutation word in sHotLo instead and expand the winner's S' in the flush: per pod, not per node.
     __shared__ uint32_t sHotLo[SP_THREADS], sHotHi[STREAM ? 1 : SP_THREADS];
@@ -408,7 +423,7 @@ score_pairs_sparse(const int4 *__restrict__ rec, const uint32_t *__restrict__ me
 #endif
 
     const int tid = threadIdx.x;
-    SpEnt *const tab = sTab[tid >> 5];
+    uint32_t *const best_row = sTab.best[tid >> 5];
     const uint32_t lane_field = (uint32_t)(tid & 31) << 8;
 
     // ---- staging: the node's compacted pair costs (7 x 16 B), permutation and free count ----------
@@ -535,60 +550,63 @@ score_pairs_sparse(const int4 *__restrict__ rec, const uint32_t *__restrict__ me
         __syncthreads();
         if (tid < NB) sCnt[tid] = 0;
         __syncthreads();
-        for (int i = tid; i < cn; i += SP_THREADS) {
-            const int4 req = __ldg(pods4 + c0 + i);
-            const bool wants_mem = req.w > 0;
-            int b = 9 * SUB;
-            if (req.x >= 0 && req.x <= 8 && wants_mem == MEM)
-                b = req.x * SUB + (MEM ? (int)(((uint32_t)req.w * 0x9E3779B1u) >> 30) : 0);
-            sK[i] = (uint8_t)b;
-            atomicAdd(&sCnt[b], 1);
+        // each thread keeps its pods' buckets and multipliers in registers from the count to the scatter
+        int bkt[PPT];
+        uint32_t mult[PPT];
+#pragma unroll
+        for (int u = 0; u < PPT; u++) {
+            const int i = tid + u * SP_THREADS;
+            bkt[u] = 9 * SUB;
+            mult[u] = 0;
+            if (i < cn) {
+                const int4 req = __ldg(pods4 + c0 + i);
+                const bool wants_mem = req.w > 0;
+                if (req.x >= 0 && req.x <= 8 && wants_mem == MEM)
+                    bkt[u] = req.x * SUB + (MEM ? (int)(((uint32_t)req.w * 0x9E3779B1u) >> 30) : 0);
+                // the per-pod multiplier: the pod's own k less what its bucket adds back (= 1 at run time)
+                mult[u] = MEM ? (uint32_t)req.w : (uint32_t)(req.x - (bkt[u] < 9 ? bkt[u] - 1 : 0));
+                atomicAdd(&sCnt[bkt[u]], 1);
+            }
         }
         __syncthreads();
-        if (tid == 0) {                            // sOff[k]: where k's pods start (a group boundary); sCnt: running positions
-            int acc = 0;
-#pragma unroll 1
-            for (int k = 0; k < 9; k++) {
+        if (tid < 32) {                            // warp 0, lane k: bucket k.  sOff[k]: where k's pods start; sCnt: running positions
+            const int k = tid;
+            int cnt[SUB], c = 0;
+#pragma unroll
+            for (int u = 0; u < SUB; u++) { cnt[u] = k < 9 ? sCnt[k * SUB + u] : 0; c += cnt[u]; }
+            const int padded = (c + SP_PAD - 1) / SP_PAD * SP_PAD;
+            int end = padded;                      // inclusive prefix sum over lanes 0..8
+#pragma unroll
+            for (int d = 1; d < 16; d <<= 1) {
+                const int t = __shfl_up_sync(0xFFFFFFFFu, end, d);
+                if (k >= d) end += t;
+            }
+            const int served = __shfl_sync(0xFFFFFFFFu, end, 8);
+            const uint32_t nonempty = __ballot_sync(0xFFFFFFFFu, c > 0);
+            if (k < 9) {
+                int acc = end - padded;
                 sOff[k] = acc;
-                for (int u = 0; u < SUB; u++) { const int c = sCnt[k * SUB + u]; sCnt[k * SUB + u] = acc; acc += c; }
-                sPad[k] = acc % SP_GROUP ? acc : -1;                 // position of k's first dummy pod, if it needs any
-                acc = (acc + SP_GROUP - 1) / SP_GROUP * SP_GROUP;
+#pragma unroll
+                for (int u = 0; u < SUB; u++) { sCnt[k * SUB + u] = acc; acc += cnt[u]; }
+                for (; acc < end; acc++) {         // dummy pods up to the next multiple of SP_PAD
+                    sIdx[acc] = SP_DUMMY;
+                    sTab.one[acc] = MEM ? 0u : 1u;
+                }
+            } else if (k == 9) {
+                sCnt[9 * SUB] = served;            // the pods not for this launch follow bucket 8
+                sOff[9] = served;
+                sOff[11] = (int)nonempty;
             }
-            sOff[9] = acc;
-            {
-                int nonempty = 0;
-#pragma unroll 1
-                for (int k = 0; k < 9; k++)
-                    if (sOff[k + 1] > sOff[k]) nonempty |= 1 << k;
-                sOff[11] = nonempty;
-            }
-            const int c9 = sCnt[9 * SUB];
-            sCnt[9 * SUB] = acc;
-            sOff[10] = acc + c9;
         }
         __syncthreads();
-        for (int i = tid; i < cn; i += SP_THREADS) {
-            const int b = sK[i];
-            const int at = atomicAdd(&sCnt[b], 1);
-            sIdx[at] = (uint16_t)i;
-            if (multi) sAcc[at] = ~0ull;
-            // the per-pod multiplier: the pod's own k less what its bucket adds back (= 1 at run time)
-            const int4 req = __ldg(pods4 + c0 + i);
-            const uint32_t one = MEM ? (uint32_t)req.w : (uint32_t)(req.x - (b < 9 ? b - 1 : 0));
 #pragma unroll
-            for (int w = 0; w < SP_WARPS; w++) {
-                sTab[w][at / SP_GROUP].one[at % SP_GROUP] = one;
-                sTab[w][at / SP_GROUP].best[at % SP_GROUP] = INF32;          // warps skip the pods they cannot serve
-            }
-        }
-        if (SP_GROUP > 1 && tid < 9 && sPad[tid] >= 0) {                   // k's padding: dummy pods up to the group boundary
-            for (int at = sPad[tid]; at % SP_GROUP != 0; at++) {
-                sIdx[at] = SP_DUMMY;
-#pragma unroll
-                for (int w = 0; w < SP_WARPS; w++) {
-                    sTab[w][at / SP_GROUP].one[at % SP_GROUP] = MEM ? 0u : 1u;
-                    sTab[w][at / SP_GROUP].best[at % SP_GROUP] = INF32;
-                }
+        for (int u = 0; u < PPT; u++) {
+            const int i = tid + u * SP_THREADS;
+            if (i < cn) {
+                const int at = atomicAdd(&sCnt[bkt[u]], 1);
+                sIdx[at] = (uint16_t)i;
+                if (multi) sAcc[at] = ~0ull;
+                sTab.one[at] = mult[u];
             }
         }
         __syncthreads();
@@ -598,7 +616,7 @@ score_pairs_sparse(const int4 *__restrict__ rec, const uint32_t *__restrict__ me
         // word says which buckets to enter
         const uint32_t kmask = STREAM ? (uint32_t)sOff[11] : 0x1FFu;
 #define KGPU_SP_RUN(K) \
-        if (!STREAM || ((kmask >> K) & 1u)) sp_run_k<K, PER_PAIR, MEM, BYTE_KEYS>(F, C, pc, nfree, valid, mem, lane_field, tab, sOff[K], sOff[K + 1]);
+        if (!STREAM || ((kmask >> K) & 1u)) sp_run_k<K, PER_PAIR, MEM, BYTE_KEYS>(F, C, pc, nfree, valid, mem, lane_field, sTab.one, best_row, sOff[K], sOff[K + 1]);
         KGPU_SP_RUN(0) KGPU_SP_RUN(1) KGPU_SP_RUN(2) KGPU_SP_RUN(3) KGPU_SP_RUN(4) KGPU_SP_RUN(5) KGPU_SP_RUN(6) KGPU_SP_RUN(7) KGPU_SP_RUN(8)
 #undef KGPU_SP_RUN
         __syncthreads();
@@ -609,18 +627,18 @@ score_pairs_sparse(const int4 *__restrict__ rec, const uint32_t *__restrict__ me
         // otherwise (a tile of two classes) node ids are compared explicitly.
         const int served = sOff[9];                // bucket 9 (not for this launch) sits at the end
         for (int i = tid; i < served; i += SP_THREADS) {
-            if (SP_GROUP > 1 && sIdx[i] == SP_DUMMY) continue;
+            if (sIdx[i] == SP_DUMMY) continue;
             uint32_t best_m = INF32, cost = 0;
             int best_slot = -1;
             if (BYTE_KEYS && ordered) {
 #pragma unroll
-                for (int w = 0; w < SP_WARPS; w++) best_m = min(best_m, sTab[w][i / SP_GROUP].best[i % SP_GROUP] | ((uint32_t)w << 13));   // INF32 stays INF32
+                for (int w = 0; w < SP_WARPS; w++) best_m = min(best_m, sTab.best[w][i] | ((uint32_t)w << 13));   // INF32 stays INF32
                 if (best_m != INF32) { best_slot = (int)((best_m >> 8) & (uint32_t)(SP_THREADS - 1)); cost = best_m >> 16; }
             } else {
                 unsigned long long best = ~0ull;   // cost<<32 | node index
 #pragma unroll
                 for (int w = 0; w < SP_WARPS; w++) {
-                    const uint32_t m = sTab[w][i / SP_GROUP].best[i % SP_GROUP];
+                    const uint32_t m = sTab.best[w][i];
                     if (m == INF32) continue;
                     const int s = w * 32 + (int)((m >> 8) & 31u);
                     const unsigned long long cand = ((unsigned long long)(m >> (BYTE_KEYS ? 16 : 13)) << 32) | (uint32_t)sNode[s];
@@ -651,10 +669,6 @@ score_pairs_sparse(const int4 *__restrict__ rec, const uint32_t *__restrict__ me
                 const unsigned long long nid = (unsigned long long)(node_id_base + (long long)sNode[best_slot]);
                 const unsigned long long key = ((unsigned long long)cost << 40) | (nid << 8) | S;
                 atomicMin(&keys[c0 + sIdx[i]], key);
-            }
-            if (multi) {                                     // the next tile starts from "no result" again
-#pragma unroll
-                for (int w = 0; w < SP_WARPS; w++) sTab[w][i / SP_GROUP].best[i % SP_GROUP] = INF32;
             }
         }
     }

@@ -26,7 +26,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--seconds", type=float, default=300)
     ap.add_argument("--seed", type=int, default=1)
-    ap.add_argument("--define", action="append", default=[], help="build knob for a private emulation build, e.g. KGPU_SP_GROUP=4")
+    ap.add_argument("--define", action="append", default=[], help="build knob for a private emulation build, e.g. KGPU_SP_UNROLL=2")
     a = ap.parse_args()
     emu_dir = os.path.join(ROOT, "tests", "emu")
     if a.define:
