@@ -15,6 +15,7 @@
 #include <unordered_set>
 #include <vector>
 
+#include "buffer.h"
 #include "multi_device.h"
 #include "place_sequential.cuh"
 #include "preempt.cuh"
@@ -42,61 +43,52 @@ struct kgpu_shard {
     int sm_count = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    int32_t *d_topo = nullptr;       // [n][64]
-    int32_t *d_free = nullptr;       // [n]
-    int32_t *d_mem = nullptr;        // [n][8] MiB per GPU (0x7F7F7F7F = unconstrained until uploaded)
-    int *d_flag = nullptr;           // "batch has memory-constrained pods"
-    int4 *d_rec = nullptr;           // K1s: [tiles][7][SP_THREADS] compacted scaled pair costs, slot order (compact_nodes)
-    uint32_t *d_meta = nullptr;      // K1s: [n_slots] position -> GPU index (3-bit fields) | free count << 24
+    kgpu::DeviceBuffer<int32_t> d_topo;   // [n][64]
+    kgpu::DeviceBuffer<int32_t> d_free;   // [n]
+    kgpu::DeviceBuffer<int32_t> d_mem;    // [n][8] MiB per GPU (0x7F7F7F7F = unconstrained until uploaded)
+    kgpu::DeviceBuffer<int> d_flag;       // "batch has memory-constrained pods"
+    kgpu::DeviceBuffer<int4> d_rec;       // K1s: [tiles][7][SP_THREADS] compacted scaled pair costs, slot order (compact_nodes)
+    kgpu::DeviceBuffer<uint32_t> d_meta;  // K1s: [n_slots] position -> GPU index (3-bit fields) | free count << 24
     bool compact_dirty = true;       // topology / weights changed for every node since the cache was built
     bool order_dirty = true;         // the order (slots by free count) must be rebuilt before the next K1s launch
     int64_t stale_nodes = 0;         // nodes whose free count changed since the order was built (re-sort when many)
-    int32_t *d_order = nullptr;      // K1s: slot -> node index, grouped by popcount(free), -1 = padding
-    int32_t *d_slot_of = nullptr;    // K1s: node index -> slot
-    int32_t *d_ord_cnt = nullptr, *d_ord_off = nullptr;   // counting sort scratch [9][blocks]
-    long long *d_ord_meta = nullptr; // class counts [9], n_slots
-    int64_t ord_nb_cap = 0;
-    unsigned long long *d_bad = nullptr;   // validate_topo_dev: first out-of-domain element
-    int32_t *d_upd = nullptr;        // state-change scratch: [cap] node indices | [cap] masks
-    uint32_t *d_fit_patch = nullptr; // [9][cap] fit-table rows of the nodes a state change touched
-    int64_t upd_cap = 0;
-    uint32_t *d_fit = nullptr;       // (node, k) fit table on the device [9][n] and, patches, [9][upd]
-    uint32_t *h_fit = nullptr;       // pinned host copy [9][n]: kgpu_fit_lookup / kgpu_score_pairs read it
-    int64_t fit_cap = 0;
+    kgpu::DeviceBuffer<int32_t> d_order;     // K1s: slot -> node index, grouped by popcount(free), -1 = padding
+    kgpu::DeviceBuffer<int32_t> d_slot_of;   // K1s: node index -> slot
+    kgpu::DeviceBuffer<int32_t> d_ord_cnt, d_ord_off;   // counting sort scratch [9][blocks]
+    kgpu::DeviceBuffer<long long> d_ord_meta;           // class counts [9], n_slots
+    kgpu::DeviceBuffer<unsigned long long> d_bad;       // validate_topo_dev: first out-of-domain element
+    kgpu::DeviceBuffer<int32_t> d_upd;        // state-change scratch: [m] node indices | [m] masks
+    kgpu::DeviceBuffer<uint32_t> d_fit_patch; // [9][m] fit-table rows of the nodes a state change touched
+    kgpu::DeviceBuffer<uint32_t> d_fit;       // (node, k) fit table on the device [9][n]
+    kgpu::PinnedBuffer<uint32_t> h_fit;       // pinned host copy [9][n]: kgpu_fit_lookup / kgpu_score_pairs read it
     bool fit_valid = false;
-    int4 *d_query = nullptr;         // kgpu_score_pairs with min_mem: {node lo, node hi, k, min_mem}
-    uint32_t *d_qout = nullptr;
-    int64_t query_cap = 0;
-    int32_t *d_free_scratch = nullptr;   // kgpu_place_batch_ex(KGPU_PLACE_DRY_RUN): the masks the dry run consumes
-    int32_t *d_hold = nullptr;       // [n][8] holder table (kgpu_upload_holders / kgpu_set_holders), allocated on first upload
-    int64_t hold_cap = 0;
+    kgpu::DeviceBuffer<int4> d_query;         // kgpu_score_pairs with min_mem: {node lo, node hi, k, min_mem}
+    kgpu::DeviceBuffer<uint32_t> d_qout;
+    kgpu::DeviceBuffer<int32_t> d_free_scratch;   // kgpu_place_batch_ex(KGPU_PLACE_DRY_RUN): the masks the dry run consumes
+    kgpu::DeviceBuffer<int32_t> d_hold;       // [n][8] holder table (kgpu_upload_holders / kgpu_set_holders), allocated on first upload
     bool has_hold = false;           // false = every entry is -1 (no upload since the last kgpu_upload_nodes)
-    int32_t *d_lvl = nullptr;        // kgpu_preempt_batch scratch [pre_cap]: pod levels, compacted pod positions,
-    int32_t *d_pidx = nullptr;       //   their preemption keys, victims, and the compacted count
-    unsigned long long *d_pkey = nullptr;
-    uint32_t *d_victims = nullptr;
-    int *d_pcnt = nullptr;
-    int64_t pre_cap = 0;
-    int64_t free_scratch_cap = 0;
+    kgpu::DeviceBuffer<int32_t> d_lvl;        // kgpu_preempt_batch scratch [P]: pod levels, compacted pod positions,
+    kgpu::DeviceBuffer<int32_t> d_pidx;       //   their preemption keys, victims, and the compacted count
+    kgpu::DeviceBuffer<unsigned long long> d_pkey;
+    kgpu::DeviceBuffer<uint32_t> d_victims;
+    kgpu::DeviceBuffer<int> d_pcnt;
     int64_t class_count[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-    int64_t n_slots = 0, slot_cap = 0;
-    int64_t n = 0, cap = 0;
+    int64_t n_slots = 0;
+    int64_t n = 0;
     int64_t node_id_base = 0;
-    int32_t *d_pods = nullptr;       // [pcap][4]
-    int32_t *d_gang = nullptr;       // [pcap] kgpu_place_batch_gang: gang id per pod
-    unsigned long long *d_keys = nullptr;    // [pcap]
-    unsigned long long *d_gather = nullptr;  // [ndev][pcap] (multi-device only)
-    unsigned long long *d_bestk = nullptr;   // [9] memo variant
+    kgpu::DeviceBuffer<int32_t> d_pods;       // [P][4]
+    kgpu::DeviceBuffer<int32_t> d_gang;       // [P] kgpu_place_batch_gang: gang id per pod
+    kgpu::DeviceBuffer<unsigned long long> d_keys;     // [P]
+    kgpu::DeviceBuffer<unsigned long long> d_gather;   // [ndev][P] (multi-device only)
+    kgpu::DeviceBuffer<unsigned long long> d_bestk;    // [9] memo variant
     std::vector<uint8_t> tile_class;         // K1s: max free-GPU count per 128-slot tile of the order (host copy)
     std::vector<kgpu::SparseWorkItem> h_work;   // K1s work list for work_P pods (sparse_work.h)
-    int4 *d_work = nullptr;
-    int64_t work_cap = 0, work_P = -1;
+    kgpu::DeviceBuffer<int4> d_work;
+    int64_t work_P = -1;
     bool tma_attr_done = false;                 // cudaFuncSetAttribute of the TMA instantiations done on this device
-    uint32_t *d_nodebest = nullptr;          // [views][9][Npad]  K3 tables
-    int32_t *d_half = nullptr;               // [Npad][96]  K3: half tables of every node (place_half_tables)
-    unsigned long long *d_tilebest = nullptr;   // [views][9][T]
-    int64_t place_cap = 0;
-    int64_t pcap = 0;
+    kgpu::DeviceBuffer<uint32_t> d_nodebest;    // [views][9][Npad]  K3 tables
+    kgpu::DeviceBuffer<int32_t> d_half;         // [Npad][96]  K3: half tables of every node (place_half_tables)
+    kgpu::DeviceBuffer<unsigned long long> d_tilebest;   // [views][9][T]
 };
 
 struct kgpu_ctx {
@@ -116,10 +108,10 @@ struct kgpu_ctx {
     struct {
         int world = 0, rank = 0;
         int64_t max_pods = 0;
-        void *base = nullptr;
+        kgpu::DeviceBuffer<unsigned char> base;
         void *peer_base[kgpu::PEER_MAX_WORLD] = {};
-        unsigned long long *local = nullptr;
-        unsigned long long *final_keys = nullptr;   // [2][max_pods]: the global keys of the last two epochs
+        kgpu::DeviceBuffer<unsigned long long> local;
+        kgpu::DeviceBuffer<unsigned long long> final_keys;   // [2][max_pods]: the global keys of the last two epochs
         uint32_t epoch = 0;
         bool connected = false;
     } xch;
@@ -165,20 +157,18 @@ int upload_subset_tables(kgpu_ctx *h) {
     return KGPU_OK;
 }
 
-int ensure_pod_capacity(kgpu_ctx *h, kgpu_shard &s, int64_t P) {
-    if (P <= s.pcap) return KGPU_OK;
-    int64_t cap = std::max<int64_t>(1024, P + P / 4);
+// Scratch sized by a call's batch grows with headroom, so that a slowly growing batch reallocates rarely: pod-indexed
+// buffers to P + P / 4 pods (at least 1024), the update and query lists to m + m / 2 entries (at least 256).
+int64_t pod_headroom(int64_t P) { return std::max<int64_t>(1024, P + P / 4); }
+int64_t list_headroom(int64_t m) { return std::max<int64_t>(256, m + m / 2); }
+
+// The pods and keys of a P-pod batch on shard s, and with several devices the all-gather's receive buffer.
+int reserve_pods(kgpu_ctx *h, kgpu_shard &s, int64_t P) {
+    const int64_t cap = pod_headroom(P), G = (int64_t)h->shards.size();
     KGPU_CUDA(h, cudaSetDevice(s.dev));
-    if (s.d_pods) cudaFree(s.d_pods);
-    if (s.d_gang) cudaFree(s.d_gang);
-    if (s.d_keys) cudaFree(s.d_keys);
-    if (s.d_gather) cudaFree(s.d_gather);
-    s.d_pods = nullptr; s.d_gang = nullptr; s.d_keys = nullptr; s.d_gather = nullptr; s.pcap = 0;
-    KGPU_CUDA(h, cudaMalloc(&s.d_pods, (size_t)cap * 16));
-    KGPU_CUDA(h, cudaMalloc(&s.d_gang, (size_t)cap * 4));
-    KGPU_CUDA(h, cudaMalloc(&s.d_keys, (size_t)cap * 8));
-    if (h->shards.size() > 1) KGPU_CUDA(h, cudaMalloc(&s.d_gather, (size_t)cap * 8 * h->shards.size()));
-    s.pcap = cap;
+    KGPU_CUDA(h, s.d_pods.reserve(4 * P, 4 * cap));
+    KGPU_CUDA(h, s.d_keys.reserve(P, cap));
+    if (G > 1) KGPU_CUDA(h, s.d_gather.reserve(G * P, G * cap));
     return KGPU_OK;
 }
 
@@ -192,29 +182,16 @@ const int kOrderPad = [] { const char *e = getenv("KGPU_ORDER_PAD"); const int v
 int build_order(kgpu_ctx *h, kgpu_shard &s) {
     KGPU_CUDA(h, cudaSetDevice(s.dev));
     const int64_t need_slots = s.n + 10 * kgpu::SP_THREADS;
-    if (need_slots > s.slot_cap) {
-        if (s.d_order) cudaFree(s.d_order);
-        if (s.d_rec) cudaFree(s.d_rec);
-        if (s.d_meta) cudaFree(s.d_meta);
-        s.d_order = nullptr; s.d_rec = nullptr; s.d_meta = nullptr; s.slot_cap = 0;
-        const int64_t cap = (need_slots + kgpu::SP_THREADS - 1) / kgpu::SP_THREADS * kgpu::SP_THREADS;
-        KGPU_CUDA(h, cudaMalloc(&s.d_order, (size_t)cap * 4));
-        KGPU_CUDA(h, cudaMalloc(&s.d_meta, (size_t)cap * 4));
-        KGPU_CUDA(h, cudaMalloc(&s.d_rec, (size_t)cap * 112));
-        s.slot_cap = cap;
-    }
+    const int64_t slots = (need_slots + kgpu::SP_THREADS - 1) / kgpu::SP_THREADS * kgpu::SP_THREADS;
+    KGPU_CUDA(h, s.d_order.reserve(need_slots, slots));
+    KGPU_CUDA(h, s.d_meta.reserve(need_slots, slots));
+    KGPU_CUDA(h, s.d_rec.reserve(7 * need_slots, 7 * slots));
     const int nb = (int)((s.n + kgpu::ORD_BLOCK - 1) / kgpu::ORD_BLOCK);
-    if (nb > s.ord_nb_cap) {
-        if (s.d_ord_cnt) cudaFree(s.d_ord_cnt);
-        if (s.d_ord_off) cudaFree(s.d_ord_off);
-        s.d_ord_cnt = nullptr; s.d_ord_off = nullptr; s.ord_nb_cap = 0;
-        KGPU_CUDA(h, cudaMalloc(&s.d_ord_cnt, (size_t)nb * 9 * 4));
-        KGPU_CUDA(h, cudaMalloc(&s.d_ord_off, (size_t)nb * 9 * 4));
-        s.ord_nb_cap = nb;
-    }
+    KGPU_CUDA(h, s.d_ord_cnt.reserve(9 * nb));
+    KGPU_CUDA(h, s.d_ord_off.reserve(9 * nb));
     long long meta[kgpu::ORD_META] = {0};
     if (s.n > 0) {
-        KGPU_CUDA(h, cudaMemsetAsync(s.d_order, 0xFF, (size_t)s.slot_cap * 4, s.stream));
+        KGPU_CUDA(h, cudaMemsetAsync(s.d_order, 0xFF, (size_t)s.d_order.capacity() * 4, s.stream));
         kgpu::order_count<<<nb, kgpu::ORD_BLOCK, 0, s.stream>>>(s.d_free, s.n, s.d_ord_cnt, nb);
         kgpu::order_scan<<<1, kgpu::ORD_BLOCK, 0, s.stream>>>(s.d_ord_cnt, nb, s.d_ord_off, s.d_ord_meta, kgpu::SP_THREADS, kOrderPad);
         kgpu::order_scatter<<<nb, kgpu::ORD_BLOCK, 0, s.stream>>>(s.d_free, s.n, s.d_ord_off, nb, s.d_order, s.d_slot_of);
@@ -262,7 +239,7 @@ int ensure_node_cache(kgpu_ctx *h, kgpu_shard &s) {
         kgpu::Weights W;
         memcpy(W.w, h->W, sizeof W.w);
         kgpu::compact_nodes<<<(unsigned)(s.n_slots / kgpu::SP_THREADS), kgpu::SP_THREADS, 0, s.stream>>>(
-            reinterpret_cast<const int4 *>(s.d_topo), s.d_free, s.n_slots, W, s.d_order, s.d_slot_of, s.d_rec, s.d_meta);
+            reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_free, s.n_slots, W, s.d_order, s.d_slot_of, s.d_rec, s.d_meta);
         h->launches++;
         KGPU_CUDA(h, cudaGetLastError());
     }
@@ -271,33 +248,15 @@ int ensure_node_cache(kgpu_ctx *h, kgpu_shard &s) {
     return KGPU_OK;
 }
 
-int ensure_upd_capacity(kgpu_ctx *h, kgpu_shard &s, int64_t m) {
-    if (m <= s.upd_cap) return KGPU_OK;
-    if (s.d_upd) cudaFree(s.d_upd);
-    if (s.d_fit_patch) cudaFree(s.d_fit_patch);
-    s.d_upd = nullptr; s.d_fit_patch = nullptr; s.upd_cap = 0;
-    const int64_t cap = std::max<int64_t>(256, m + m / 2);
-    KGPU_CUDA(h, cudaMalloc(&s.d_upd, (size_t)cap * 8));
-    KGPU_CUDA(h, cudaMalloc(&s.d_fit_patch, (size_t)cap * 36));
-    s.upd_cap = cap;
-    return KGPU_OK;
-}
-
 // (node, k) fit table of shard s: fit_nodes over every node, one copy to the pinned host array.
 int build_fit_table(kgpu_ctx *h, kgpu_shard &s) {
     KGPU_CUDA(h, cudaSetDevice(s.dev));
-    if (s.n > s.fit_cap) {
-        if (s.d_fit) cudaFree(s.d_fit);
-        if (s.h_fit) cudaFreeHost(s.h_fit);
-        s.d_fit = nullptr; s.h_fit = nullptr; s.fit_cap = 0;
-        KGPU_CUDA(h, cudaMalloc(&s.d_fit, (size_t)s.n * 36));
-        KGPU_CUDA(h, cudaMallocHost(&s.h_fit, (size_t)s.n * 36));
-        s.fit_cap = s.n;
-    }
+    KGPU_CUDA(h, s.d_fit.reserve(9 * s.n));
+    KGPU_CUDA(h, s.h_fit.reserve(9 * s.n));
     if (s.n > 0) {
         kgpu::Weights W;
         memcpy(W.w, h->W, sizeof W.w);
-        kgpu::fit_nodes<<<(unsigned)((s.n + 127) / 128), 128, 0, s.stream>>>(reinterpret_cast<const int4 *>(s.d_topo), s.d_free,
+        kgpu::fit_nodes<<<(unsigned)((s.n + 127) / 128), 128, 0, s.stream>>>(reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_free,
                                                                           nullptr, s.n, W, PC, s.d_fit);
         h->launches++;
         KGPU_CUDA(h, cudaGetLastError());
@@ -314,26 +273,27 @@ int build_fit_table(kgpu_ctx *h, kgpu_shard &s) {
 int apply_node_updates(kgpu_ctx *h, kgpu_shard &s, const int32_t *idx, const int32_t *masks, int64_t m) {
     if (m <= 0) return KGPU_OK;
     KGPU_CUDA(h, cudaSetDevice(s.dev));
-    int rc = ensure_upd_capacity(h, s, m);
-    if (rc != KGPU_OK) return rc;
+    KGPU_CUDA(h, s.d_upd.reserve(2 * m, 2 * list_headroom(m)));
+    if (s.fit_valid) KGPU_CUDA(h, s.d_fit_patch.reserve(9 * m, 9 * list_headroom(m)));
+    int32_t *d_masks = masks ? s.d_upd + m : nullptr;
     KGPU_CUDA(h, cudaMemcpyAsync(s.d_upd, idx, (size_t)m * 4, cudaMemcpyHostToDevice, s.stream));
-    if (masks) KGPU_CUDA(h, cudaMemcpyAsync(s.d_upd + s.upd_cap, masks, (size_t)m * 4, cudaMemcpyHostToDevice, s.stream));
+    if (masks) KGPU_CUDA(h, cudaMemcpyAsync(d_masks, masks, (size_t)m * 4, cudaMemcpyHostToDevice, s.stream));
     kgpu::Weights W;
     memcpy(W.w, h->W, sizeof W.w);
-    const int4 *topo4 = reinterpret_cast<const int4 *>(s.d_topo);
+    const int4 *topo4 = reinterpret_cast<const int4 *>(s.d_topo.get());
     const bool cache_live = !s.order_dirty && !s.compact_dirty;
     if (cache_live) {
         kgpu::compact_nodes<<<(unsigned)((m + kgpu::SP_THREADS - 1) / kgpu::SP_THREADS), kgpu::SP_THREADS, 0, s.stream>>>(
-            topo4, s.d_free, m, W, s.d_order, s.d_slot_of, s.d_rec, s.d_meta, s.d_upd, masks ? s.d_upd + s.upd_cap : nullptr);
+            topo4, s.d_free, m, W, s.d_order, s.d_slot_of, s.d_rec, s.d_meta, s.d_upd, d_masks);
         h->launches++;
         s.stale_nodes += m;
     } else if (masks) {
-        kgpu::scatter_masks<<<(unsigned)((m + 255) / 256), 256, 0, s.stream>>>(s.d_upd, s.d_upd + s.upd_cap, m, s.d_free);
+        kgpu::scatter_masks<<<(unsigned)((m + 255) / 256), 256, 0, s.stream>>>(s.d_upd, d_masks, m, s.d_free);
         h->launches++;
     }
     KGPU_CUDA(h, cudaGetLastError());
     if (s.fit_valid) {
-        // rows of the changed nodes -> the persistent patch buffer (grown with the index scratch) -> the host table
+        // rows of the changed nodes -> the persistent patch buffer -> the host table
         kgpu::fit_nodes<<<(unsigned)((m + 127) / 128), 128, 0, s.stream>>>(topo4, s.d_free, s.d_upd, m, W, PC, s.d_fit_patch);
         h->launches++;
         KGPU_CUDA(h, cudaGetLastError());
@@ -358,10 +318,10 @@ int launch_score(kgpu_ctx *h, kgpu_shard &s, const int32_t *d_pods, int64_t P, u
     KGPU_CUDA(h, cudaSetDevice(s.dev));
     kgpu::Weights W;
     memcpy(W.w, h->W, sizeof W.w);
-    const int4 *topo4 = reinterpret_cast<const int4 *>(s.d_topo);
+    const int4 *topo4 = reinterpret_cast<const int4 *>(s.d_topo.get());
     const int4 *pods4 = reinterpret_cast<const int4 *>(d_pods);
 
-    const int4 *mem4 = reinterpret_cast<const int4 *>(s.d_mem);
+    const int4 *mem4 = reinterpret_cast<const int4 *>(s.d_mem.get());
     if (!keys_are_clean) KGPU_CUDA(h, cudaMemsetAsync(d_keys, 0xFF, (size_t)P * 8, st));
     if (s.n == 0) return KGPU_OK;
 
@@ -441,12 +401,7 @@ int launch_score(kgpu_ctx *h, kgpu_shard &s, const int32_t *d_pods, int64_t P, u
                                              : P <= kgpu::kSparseChunk               ? (int64_t)s.sm_count * KGPU_SP_STREAM_MINBLOCKS
                                                                                      : resident;
                     kgpu::build_sparse_work(s.tile_class, P, res_list, s.h_work, prm);
-                    if ((int64_t)s.h_work.size() > s.work_cap) {
-                        if (s.d_work) cudaFree(s.d_work);
-                        s.d_work = nullptr; s.work_cap = 0;
-                        KGPU_CUDA(h, cudaMalloc(&s.d_work, s.h_work.size() * sizeof(int4)));
-                        s.work_cap = (int64_t)s.h_work.size();
-                    }
+                    KGPU_CUDA(h, s.d_work.reserve((int64_t)s.h_work.size()));
                     static_assert(sizeof(kgpu::SparseWorkItem) == sizeof(int4), "work item layout");
                     KGPU_CUDA(h, cudaMemcpyAsync(s.d_work, s.h_work.data(), s.h_work.size() * sizeof(int4), cudaMemcpyHostToDevice, st));
                     s.work_P = P;
@@ -517,44 +472,10 @@ kgpu_shard *shard_of(kgpu_ctx *h, int64_t idx, int64_t *local) {
 void free_shard(kgpu_shard &s) {
     if (s.dev < 0) return;
     cudaSetDevice(s.dev);
-    if (s.d_topo) cudaFree(s.d_topo);
-    if (s.d_free) cudaFree(s.d_free);
-    if (s.d_mem) cudaFree(s.d_mem);
-    if (s.d_flag) cudaFree(s.d_flag);
-    if (s.d_order) cudaFree(s.d_order);
-    if (s.d_rec) cudaFree(s.d_rec);
-    if (s.d_meta) cudaFree(s.d_meta);
-    if (s.d_slot_of) cudaFree(s.d_slot_of);
-    if (s.d_ord_cnt) cudaFree(s.d_ord_cnt);
-    if (s.d_ord_off) cudaFree(s.d_ord_off);
-    if (s.d_ord_meta) cudaFree(s.d_ord_meta);
-    if (s.d_bad) cudaFree(s.d_bad);
-    if (s.d_upd) cudaFree(s.d_upd);
-    if (s.d_fit_patch) cudaFree(s.d_fit_patch);
-    if (s.d_fit) cudaFree(s.d_fit);
-    if (s.h_fit) cudaFreeHost(s.h_fit);
-    if (s.d_free_scratch) cudaFree(s.d_free_scratch);
-    if (s.d_hold) cudaFree(s.d_hold);
-    if (s.d_lvl) cudaFree(s.d_lvl);
-    if (s.d_pidx) cudaFree(s.d_pidx);
-    if (s.d_pkey) cudaFree(s.d_pkey);
-    if (s.d_victims) cudaFree(s.d_victims);
-    if (s.d_pcnt) cudaFree(s.d_pcnt);
-    if (s.d_query) cudaFree(s.d_query);
-    if (s.d_qout) cudaFree(s.d_qout);
-    if (s.d_pods) cudaFree(s.d_pods);
-    if (s.d_gang) cudaFree(s.d_gang);
-    if (s.d_keys) cudaFree(s.d_keys);
-    if (s.d_gather) cudaFree(s.d_gather);
-    if (s.d_bestk) cudaFree(s.d_bestk);
-    if (s.d_nodebest) cudaFree(s.d_nodebest);
-    if (s.d_tilebest) cudaFree(s.d_tilebest);
-    if (s.d_half) cudaFree(s.d_half);
-    if (s.d_work) cudaFree(s.d_work);
     if (s.ev0) cudaEventDestroy(s.ev0);
     if (s.ev1) cudaEventDestroy(s.ev1);
     if (s.stream) cudaStreamDestroy(s.stream);
-    s = kgpu_shard();
+    s = kgpu_shard();                  // frees the buffers
 }
 
 }  // namespace
@@ -601,10 +522,10 @@ int kgpu_create(const int *dev_ids, int ndev, kgpu_t **out) {
         step(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking), "cudaStreamCreate");
         step(cudaEventCreate(&s.ev0), "cudaEventCreate");
         step(cudaEventCreate(&s.ev1), "cudaEventCreate");
-        step(cudaMalloc(&s.d_bestk, 9 * 8), "cudaMalloc");
-        step(cudaMalloc(&s.d_flag, sizeof(int)), "cudaMalloc");
-        step(cudaMalloc(&s.d_ord_meta, kgpu::ORD_META * sizeof(long long)), "cudaMalloc");
-        step(cudaMalloc(&s.d_bad, sizeof(unsigned long long)), "cudaMalloc");
+        step(s.d_bestk.reserve(9), "cudaMalloc");
+        step(s.d_flag.reserve(1), "cudaMalloc");
+        step(s.d_ord_meta.reserve(kgpu::ORD_META), "cudaMalloc");
+        step(s.d_bad.reserve(1), "cudaMalloc");
     }
     if (rc == KGPU_OK && ndev > 1) {
         std::vector<int> devs(dev_ids, dev_ids + ndev);
@@ -631,13 +552,9 @@ int kgpu_destroy(kgpu_t *h) {
         if (s.dev >= 0) { cudaSetDevice(s.dev); cudaStreamSynchronize(s.stream); }
     }
     delete h->multi;
-    if (h->xch.base) {
+    if (h->xch.connected)              // unmap the peers' exchange memory before this rank's is freed (delete h)
         for (int r = 0; r < h->xch.world; r++)
-            if (h->xch.connected && r != h->xch.rank && h->xch.peer_base[r]) cudaIpcCloseMemHandle(h->xch.peer_base[r]);
-        cudaFree(h->xch.base);
-        cudaFree(h->xch.local);
-        cudaFree(h->xch.final_keys);
-    }
+            if (r != h->xch.rank && h->xch.peer_base[r]) cudaIpcCloseMemHandle(h->xch.peer_base[r]);
     for (auto &s : h->shards) free_shard(s);
     delete h;
     return KGPU_OK;
@@ -670,59 +587,29 @@ int kgpu_set_variant(kgpu_t *h, int variant) {
     return KGPU_OK;
 }
 
-int kgpu_upload_nodes(kgpu_t *h, const int32_t *topo, const int32_t *free_mask, int64_t n, int64_t node_id_base) {
-    if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_nodes: NULL handle");
-    std::lock_guard<std::mutex> g(h->mu);
-    if (n < 0 || (n > 0 && (!topo || !free_mask))) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_nodes: bad arguments");
-    if (node_id_base < 0 || node_id_base + n > 0xFFFFFFFFLL)
-        return fail(h, KGPU_ERR_INVALID, "kgpu_upload_nodes: node ids must fit in 32 bits");
-    const auto t_begin = std::chrono::steady_clock::now();
-    const int64_t G = (int64_t)h->shards.size();
-    const int64_t per = (n + G - 1) / G;     // contiguous ranges: shard g holds [g*per, ...)
-    if (per > 0x7FFFFFFFLL - 4096) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_nodes: more than 2^31 nodes per device");
-    // A failure below leaves the handle EMPTY (n = 0 everywhere), never half old / half new.
-    auto empty_all = [&]() {
-        for (auto &s : h->shards) { s.n = 0; s.n_slots = 0; s.order_dirty = true; s.compact_dirty = true; s.fit_valid = false; s.work_P = -1; }
-        h->n_total = 0;
-    };
-#define KGPU_UP(expr)                                                                                 \
-    do {                                                                                              \
-        cudaError_t e__ = (expr);                                                                     \
-        if (e__ != cudaSuccess) {                                                                     \
-            empty_all();                                                                              \
-            return fail(h, e__ == cudaErrorMemoryAllocation ? KGPU_ERR_NOMEM : KGPU_ERR_CUDA,          \
-                        "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__);  \
-        }                                                                                             \
-    } while (0)
+namespace {
+// kgpu_upload_nodes after its argument checks: shard g gets the contiguous range [g * per, ...).  The caller empties
+// the handle when this fails.
+int upload_nodes(kgpu_ctx *h, const int32_t *topo, const int32_t *free_mask, int64_t n, int64_t node_id_base, int64_t per) {
     int64_t off = 0;
     for (auto &s : h->shards) {
         const int64_t cnt = std::max<int64_t>(0, std::min<int64_t>(per, n - off));
-        KGPU_UP(cudaSetDevice(s.dev));
-        if (cnt > s.cap) {
-            if (s.d_topo) cudaFree(s.d_topo);
-            if (s.d_free) cudaFree(s.d_free);
-            if (s.d_mem) cudaFree(s.d_mem);
-            if (s.d_slot_of) cudaFree(s.d_slot_of);
-            if (s.d_hold) cudaFree(s.d_hold);
-            s.d_topo = nullptr; s.d_free = nullptr; s.d_mem = nullptr; s.d_slot_of = nullptr; s.cap = 0; s.n = 0;
-            s.d_hold = nullptr; s.hold_cap = 0;
-            KGPU_UP(cudaMalloc(&s.d_topo, (size_t)cnt * 256));
-            KGPU_UP(cudaMalloc(&s.d_free, (size_t)cnt * 4));
-            KGPU_UP(cudaMalloc(&s.d_mem, (size_t)cnt * 32));
-            KGPU_UP(cudaMalloc(&s.d_slot_of, (size_t)cnt * 4));
-            s.cap = cnt;
-        }
+        KGPU_CUDA(h, cudaSetDevice(s.dev));
+        KGPU_CUDA(h, s.d_topo.reserve(64 * cnt));
+        KGPU_CUDA(h, s.d_free.reserve(cnt));
+        KGPU_CUDA(h, s.d_mem.reserve(8 * cnt));
+        KGPU_CUDA(h, s.d_slot_of.reserve(cnt));
         if (cnt > 0) {
             // per-GPU memory is unconstrained (0x7F7F7F7F MiB) until kgpu_upload_gpu_memory says otherwise
-            KGPU_UP(cudaMemsetAsync(s.d_mem, 0x7F, (size_t)cnt * 32, s.stream));
-            KGPU_UP(cudaMemcpyAsync(s.d_topo, topo + off * 64, (size_t)cnt * 256, cudaMemcpyHostToDevice, s.stream));
-            KGPU_UP(cudaMemcpyAsync(s.d_free, free_mask + off, (size_t)cnt * 4, cudaMemcpyHostToDevice, s.stream));
+            KGPU_CUDA(h, cudaMemsetAsync(s.d_mem, 0x7F, (size_t)cnt * 32, s.stream));
+            KGPU_CUDA(h, cudaMemcpyAsync(s.d_topo, topo + off * 64, (size_t)cnt * 256, cudaMemcpyHostToDevice, s.stream));
+            KGPU_CUDA(h, cudaMemcpyAsync(s.d_free, free_mask + off, (size_t)cnt * 4, cudaMemcpyHostToDevice, s.stream));
             // value-domain check on the device (levels 0..15): one 8-byte read-back instead of an O(64 N) host pass
-            KGPU_UP(cudaMemsetAsync(s.d_bad, 0xFF, sizeof(unsigned long long), s.stream));
+            KGPU_CUDA(h, cudaMemsetAsync(s.d_bad, 0xFF, sizeof(unsigned long long), s.stream));
             kgpu::validate_topo_dev<<<(unsigned)((cnt * 16 + 255) / 256), 256, 0, s.stream>>>(
-                reinterpret_cast<const int4 *>(s.d_topo), cnt * 16, s.d_bad);
+                reinterpret_cast<const int4 *>(s.d_topo.get()), cnt * 16, s.d_bad);
             h->launches++;
-            KGPU_UP(cudaGetLastError());
+            KGPU_CUDA(h, cudaGetLastError());
         }
         s.n = cnt;
         s.has_hold = false;            // a new node array has no holders
@@ -738,22 +625,40 @@ int kgpu_upload_nodes(kgpu_t *h, const int32_t *topo, const int32_t *free_mask, 
     for (auto &s : h->shards) {
         if (s.n > 0) {
             unsigned long long bad = ~0ull;
-            KGPU_UP(cudaSetDevice(s.dev));
-            KGPU_UP(cudaMemcpyAsync(&bad, s.d_bad, sizeof bad, cudaMemcpyDeviceToHost, s.stream));
-            KGPU_UP(cudaStreamSynchronize(s.stream));
+            KGPU_CUDA(h, cudaSetDevice(s.dev));
+            KGPU_CUDA(h, cudaMemcpyAsync(&bad, s.d_bad, sizeof bad, cudaMemcpyDeviceToHost, s.stream));
+            KGPU_CUDA(h, cudaStreamSynchronize(s.stream));
             if (bad != ~0ull) {
                 const long long el = (long long)bad;
-                empty_all();
                 return fail(h, KGPU_ERR_INVALID, "topo[%lld][%d] = %d outside the link-level domain 0..15",
                             (long long)(off + el / 64), (int)(el % 64), topo[(off + el / 64) * 64 + el % 64]);
             }
         }
         off += s.n;
     }
-#undef KGPU_UP
     for (auto &s : h->shards) {
         const int rc = ensure_node_cache(h, s);
-        if (rc != KGPU_OK) { empty_all(); return rc; }
+        if (rc != KGPU_OK) return rc;
+    }
+    return KGPU_OK;
+}
+}  // namespace
+
+int kgpu_upload_nodes(kgpu_t *h, const int32_t *topo, const int32_t *free_mask, int64_t n, int64_t node_id_base) {
+    if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_nodes: NULL handle");
+    std::lock_guard<std::mutex> g(h->mu);
+    if (n < 0 || (n > 0 && (!topo || !free_mask))) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_nodes: bad arguments");
+    if (node_id_base < 0 || node_id_base + n > 0xFFFFFFFFLL)
+        return fail(h, KGPU_ERR_INVALID, "kgpu_upload_nodes: node ids must fit in 32 bits");
+    const auto t_begin = std::chrono::steady_clock::now();
+    const int64_t G = (int64_t)h->shards.size();
+    const int64_t per = (n + G - 1) / G;     // contiguous ranges: shard g holds [g*per, ...)
+    if (per > 0x7FFFFFFFLL - 4096) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_nodes: more than 2^31 nodes per device");
+    const int rc = upload_nodes(h, topo, free_mask, n, node_id_base, per);
+    if (rc != KGPU_OK) {               // a failed upload leaves the handle EMPTY (n = 0 everywhere), never half old / half new
+        for (auto &s : h->shards) { s.n = 0; s.n_slots = 0; s.order_dirty = true; s.compact_dirty = true; s.fit_valid = false; s.work_P = -1; }
+        h->n_total = 0;
+        return rc;
     }
     h->last_upload_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
     return KGPU_OK;
@@ -858,7 +763,7 @@ int kgpu_score_batch(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out_ke
     if (P == 0) return KGPU_OK;
     const size_t G = h->shards.size();
     for (auto &s : h->shards) {
-        int rc = ensure_pod_capacity(h, s, P);
+        int rc = reserve_pods(h, s, P);
         if (rc != KGPU_OK) return rc;
     }
     int has_mem = 0;
@@ -939,20 +844,15 @@ int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, i
         views.min_mem[views.n++] = need;
     }
     kgpu_shard &s = h->shards[0];
-    int rc = ensure_pod_capacity(h, s, P);
+    const int rc = reserve_pods(h, s, P);
     if (rc != KGPU_OK) return rc;
-    KGPU_CUDA(h, cudaSetDevice(s.dev));
+    if (gang) KGPU_CUDA(h, s.d_gang.reserve(P, pod_headroom(P)));
     KGPU_CUDA(h, cudaMemcpyAsync(s.d_pods, pods, (size_t)P * 16, cudaMemcpyHostToDevice, s.stream));
     if (gang) KGPU_CUDA(h, cudaMemcpyAsync(s.d_gang, gang, (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
     const bool dry = (flags & KGPU_PLACE_DRY_RUN) != 0;
     int32_t *d_free = s.d_free;
     if (dry && s.n > 0) {                  // place on a scratch copy of the masks: conflict-free proposals, nothing taken
-        if (s.n > s.free_scratch_cap) {
-            if (s.d_free_scratch) cudaFree(s.d_free_scratch);
-            s.d_free_scratch = nullptr; s.free_scratch_cap = 0;
-            KGPU_CUDA(h, cudaMalloc(&s.d_free_scratch, (size_t)s.n * 4));
-            s.free_scratch_cap = s.n;
-        }
+        KGPU_CUDA(h, s.d_free_scratch.reserve(s.n));
         KGPU_CUDA(h, cudaMemcpyAsync(s.d_free_scratch, s.d_free, (size_t)s.n * 4, cudaMemcpyDeviceToDevice, s.stream));
         d_free = s.d_free_scratch;
     }
@@ -960,22 +860,14 @@ int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, i
         KGPU_CUDA(h, cudaMemsetAsync(s.d_keys, 0xFF, (size_t)P * 8, s.stream));
     } else {
         const int64_t T = (s.n + kgpu::PLACE_TILE - 1) / kgpu::PLACE_TILE, Npad = T * kgpu::PLACE_TILE;
-        if (Npad * views.n > s.place_cap) {
-            if (s.d_nodebest) cudaFree(s.d_nodebest);
-            if (s.d_tilebest) cudaFree(s.d_tilebest);
-            s.d_nodebest = nullptr; s.d_tilebest = nullptr; s.place_cap = 0;
-            KGPU_CUDA(h, cudaMalloc(&s.d_nodebest, (size_t)Npad * views.n * 9 * 4));
-            if (s.d_half) cudaFree(s.d_half);
-            s.d_half = nullptr;
-            KGPU_CUDA(h, cudaMalloc(&s.d_half, (size_t)Npad * kgpu::PLACE_HALF * 4));
-            KGPU_CUDA(h, cudaMalloc(&s.d_tilebest, (size_t)T * views.n * 9 * 8));
-            s.place_cap = Npad * views.n;
-        }
+        KGPU_CUDA(h, s.d_nodebest.reserve(Npad * views.n * 9));
+        KGPU_CUDA(h, s.d_tilebest.reserve(T * views.n * 9));
+        KGPU_CUDA(h, s.d_half.reserve(Npad * kgpu::PLACE_HALF));
         kgpu::Weights W;
         memcpy(W.w, h->W, sizeof W.w);
         KGPU_CUDA(h, cudaEventRecord(s.ev0, s.stream));
         kgpu::place_init<<<dim3((unsigned)T, (unsigned)views.n), kgpu::PLACE_TILE, 0, s.stream>>>(
-            reinterpret_cast<const int4 *>(s.d_topo), d_free, s.d_mem, s.n, Npad, s.node_id_base, W, PC, views, s.d_nodebest,
+            reinterpret_cast<const int4 *>(s.d_topo.get()), d_free, s.d_mem, s.n, Npad, s.node_id_base, W, PC, views, s.d_nodebest,
             s.d_tilebest, T);
         kgpu::place_half_tables<<<(unsigned)std::min<int64_t>((s.n + 3) / 4, (int64_t)s.sm_count * 16), 128, 0, s.stream>>>(
             s.d_topo, s.n, W, s.d_half);
@@ -985,14 +877,14 @@ int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, i
                 kgpu::place_sequential<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kgpu::PLACE_DYN_SMEM);
             KGPU_CUDA(h, place_gang_attr);
             kgpu::place_sequential<true><<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(
-                s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base, reinterpret_cast<const int4 *>(s.d_pods), P, W, views,
+                s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base, reinterpret_cast<const int4 *>(s.d_pods.get()), P, W, views,
                 s.d_nodebest, s.d_tilebest, T, s.d_half, s.d_keys, s.d_gang);
         } else {
             static const cudaError_t place_attr = cudaFuncSetAttribute(kgpu::place_sequential<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                                        (int)kgpu::PLACE_DYN_SMEM);
             KGPU_CUDA(h, place_attr);
             kgpu::place_sequential<false><<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base,
-                                                                                   reinterpret_cast<const int4 *>(s.d_pods), P, W, views,
+                                                                                   reinterpret_cast<const int4 *>(s.d_pods.get()), P, W, views,
                                                                                    s.d_nodebest, s.d_tilebest, T, s.d_half, s.d_keys);
         }
         h->launches += 2;
@@ -1036,34 +928,12 @@ int validate_holders(kgpu_ctx *h, const char *fn, const int32_t *rows, int64_t n
 // The holder table of shard s exists on the device (first use: allocated and set to all -1).
 int ensure_holders(kgpu_ctx *h, kgpu_shard &s) {
     KGPU_CUDA(h, cudaSetDevice(s.dev));
-    if (s.hold_cap < s.n) {
-        if (s.d_hold) cudaFree(s.d_hold);
-        s.d_hold = nullptr; s.hold_cap = 0; s.has_hold = false;
-        KGPU_CUDA(h, cudaMalloc(&s.d_hold, (size_t)s.n * 32));
-        s.hold_cap = s.n;
-    }
+    KGPU_CUDA(h, s.d_hold.reserve(8 * s.n));    // grows only with n, that is after kgpu_upload_nodes cleared has_hold
     if (!s.has_hold && s.n > 0) KGPU_CUDA(h, cudaMemsetAsync(s.d_hold, 0xFF, (size_t)s.n * 32, s.stream));
     s.has_hold = true;
     return KGPU_OK;
 }
 
-int ensure_preempt_capacity(kgpu_ctx *h, kgpu_shard &s, int64_t P) {
-    if (P <= s.pre_cap) return KGPU_OK;
-    const int64_t cap = std::max<int64_t>(1024, P + P / 4);
-    KGPU_CUDA(h, cudaSetDevice(s.dev));
-    if (s.d_lvl) cudaFree(s.d_lvl);
-    if (s.d_pidx) cudaFree(s.d_pidx);
-    if (s.d_pkey) cudaFree(s.d_pkey);
-    if (s.d_victims) cudaFree(s.d_victims);
-    s.d_lvl = nullptr; s.d_pidx = nullptr; s.d_pkey = nullptr; s.d_victims = nullptr; s.pre_cap = 0;
-    if (!s.d_pcnt) KGPU_CUDA(h, cudaMalloc(&s.d_pcnt, sizeof(int)));
-    KGPU_CUDA(h, cudaMalloc(&s.d_lvl, (size_t)cap * 4));
-    KGPU_CUDA(h, cudaMalloc(&s.d_pidx, (size_t)cap * 4));
-    KGPU_CUDA(h, cudaMalloc(&s.d_pkey, (size_t)cap * 8));
-    KGPU_CUDA(h, cudaMalloc(&s.d_victims, (size_t)cap * 4));
-    s.pre_cap = cap;
-    return KGPU_OK;
-}
 }  // namespace
 
 int kgpu_upload_holders(kgpu_t *h, const int32_t *holders, int64_t n) {
@@ -1108,11 +978,11 @@ int kgpu_set_holders(kgpu_t *h, const int64_t *idx, const int32_t *holders, int6
     kgpu_shard &s = h->shards[0];
     rc = ensure_holders(h, s);
     if (rc != KGPU_OK) return rc;
-    rc = ensure_upd_capacity(h, s, (int64_t)stage.size() / 2 + 1);   // d_upd holds 2 * upd_cap int32
-    if (rc != KGPU_OK) return rc;
+    const int64_t half = (int64_t)stage.size() / 2 + 1;               // d_upd is sized as two lists of this length
+    KGPU_CUDA(h, s.d_upd.reserve(2 * half, 2 * list_headroom(half)));
     KGPU_CUDA(h, cudaMemcpyAsync(s.d_upd, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, s.stream));
     kgpu::scatter_holders<<<(unsigned)((m + 255) / 256), 256, 0, s.stream>>>(
-        s.d_upd, reinterpret_cast<const int4 *>(s.d_upd + rows_off), m, reinterpret_cast<int4 *>(s.d_hold));
+        s.d_upd, reinterpret_cast<const int4 *>(s.d_upd + rows_off), m, reinterpret_cast<int4 *>(s.d_hold.get()));
     h->launches++;
     KGPU_CUDA(h, cudaGetLastError());
     KGPU_CUDA(h, cudaStreamSynchronize(s.stream));
@@ -1131,12 +1001,16 @@ int kgpu_preempt_batch(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64
     if (P == 0) return KGPU_OK;
     if (P > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_batch: more than 2^31 pods");
     kgpu_shard &s = h->shards[0];
-    int rc = ensure_pod_capacity(h, s, P);
-    if (rc == KGPU_OK) rc = ensure_preempt_capacity(h, s, P);
+    int rc = reserve_pods(h, s, P);
     if (rc != KGPU_OK) return rc;
+    const int64_t cap = pod_headroom(P);
+    KGPU_CUDA(h, s.d_lvl.reserve(P, cap));
+    KGPU_CUDA(h, s.d_pidx.reserve(P, cap));
+    KGPU_CUDA(h, s.d_pkey.reserve(P, cap));
+    KGPU_CUDA(h, s.d_victims.reserve(P, cap));
+    KGPU_CUDA(h, s.d_pcnt.reserve(1));
     int has_mem = 0;
     for (int64_t p = 0; p < P && !has_mem; p++) has_mem = pods[4 * p + 3] > 0;
-    KGPU_CUDA(h, cudaSetDevice(s.dev));
     KGPU_CUDA(h, cudaMemcpyAsync(s.d_pods, pods, (size_t)P * 16, cudaMemcpyHostToDevice, s.stream));
     KGPU_CUDA(h, cudaMemsetAsync(s.d_victims, 0, (size_t)P * 4, s.stream));
     KGPU_CUDA(h, cudaEventRecord(s.ev0, s.stream));
@@ -1145,7 +1019,7 @@ int kgpu_preempt_batch(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64
     if (rc != KGPU_OK) return rc;
     if (s.has_hold && s.n > 0) {
         // 2. the NO_FIT pods that may evict, compacted on the device; 3. K4 over them only
-        const int4 *pods4 = reinterpret_cast<const int4 *>(s.d_pods);
+        const int4 *pods4 = reinterpret_cast<const int4 *>(s.d_pods.get());
         KGPU_CUDA(h, cudaMemcpyAsync(s.d_lvl, lvl, (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
         KGPU_CUDA(h, cudaMemsetAsync(s.d_pcnt, 0, sizeof(int), s.stream));
         KGPU_CUDA(h, cudaMemsetAsync(s.d_pkey, 0xFF, (size_t)P * 8, s.stream));
@@ -1160,8 +1034,8 @@ int kgpu_preempt_batch(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64
         int64_t splits = std::max<int64_t>(1, (8 * (int64_t)s.sm_count * 4 + tiles - 1) / tiles);
         splits = std::min<int64_t>({splits, (P + kgpu::PRE_CHUNK - 1) / kgpu::PRE_CHUNK, 65535});
         kgpu::preempt_lane_per_node<<<dim3((unsigned)tiles, (unsigned)splits), kgpu::PRE_THREADS, 0, s.stream>>>(
-            reinterpret_cast<const int4 *>(s.d_topo), s.d_free, reinterpret_cast<const int4 *>(s.d_mem),
-            reinterpret_cast<const int4 *>(s.d_hold), s.n, pods4, s.d_lvl, s.d_pidx, s.d_pcnt, W, PC, s.d_pkey);
+            reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_free, reinterpret_cast<const int4 *>(s.d_mem.get()),
+            reinterpret_cast<const int4 *>(s.d_hold.get()), s.n, pods4, s.d_lvl, s.d_pidx, s.d_pcnt, W, PC, s.d_pkey);
         kgpu::preempt_finalize<<<pb, 256, 0, s.stream>>>(s.d_pkey, s.d_pidx, s.d_pcnt, s.d_free, s.d_hold, s.node_id_base,
                                                          s.d_keys, s.d_victims);
         h->launches += 3;
@@ -1252,19 +1126,11 @@ int kgpu_score_pairs(kgpu_t *h, const int64_t *node_idx, const int32_t *k, const
         if (q.empty()) continue;
         const int64_t m = (int64_t)q.size();
         KGPU_CUDA(h, cudaSetDevice(s.dev));
-        if (m > s.query_cap) {
-            if (s.d_free_scratch) cudaFree(s.d_free_scratch);
-    if (s.d_query) cudaFree(s.d_query);
-            if (s.d_qout) cudaFree(s.d_qout);
-            s.d_query = nullptr; s.d_qout = nullptr; s.query_cap = 0;
-            const int64_t cap = std::max<int64_t>(256, m + m / 2);
-            KGPU_CUDA(h, cudaMalloc(&s.d_query, (size_t)cap * 16));
-            KGPU_CUDA(h, cudaMalloc(&s.d_qout, (size_t)cap * 4));
-            s.query_cap = cap;
-        }
+        KGPU_CUDA(h, s.d_query.reserve(m, list_headroom(m)));
+        KGPU_CUDA(h, s.d_qout.reserve(m, list_headroom(m)));
         KGPU_CUDA(h, cudaMemcpyAsync(s.d_query, q.data(), (size_t)m * 16, cudaMemcpyHostToDevice, s.stream));
         kgpu::score_pair_list<<<(unsigned)((m + 127) / 128), 128, 0, s.stream>>>(
-            reinterpret_cast<const int4 *>(s.d_topo), s.d_free, s.d_mem, s.n, s.d_query, m, W, PC, s.d_qout);
+            reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_free, s.d_mem, s.n, s.d_query, m, W, PC, s.d_qout);
         h->launches++;
         KGPU_CUDA(h, cudaGetLastError());
         std::vector<uint32_t> res((size_t)m);
@@ -1316,9 +1182,9 @@ int kgpu_exchange_init(kgpu_t *h, int world, int rank, int64_t max_pods, unsigne
     if (h->xch.base) return fail(h, KGPU_ERR_STATE, "kgpu_exchange_init: already initialised");
     kgpu_shard &s = h->shards[0];
     KGPU_CUDA(h, cudaSetDevice(s.dev));
-    KGPU_CUDA(h, cudaMalloc(&h->xch.base, xch_bytes(world, max_pods)));
-    KGPU_CUDA(h, cudaMalloc(&h->xch.local, (size_t)max_pods * 8));
-    KGPU_CUDA(h, cudaMalloc(&h->xch.final_keys, (size_t)max_pods * 8 * 2));
+    KGPU_CUDA(h, h->xch.base.reserve((int64_t)xch_bytes(world, max_pods)));
+    KGPU_CUDA(h, h->xch.local.reserve(max_pods));
+    KGPU_CUDA(h, h->xch.final_keys.reserve(2 * max_pods));
     KGPU_CUDA(h, cudaMemset(h->xch.base, 0xFF, xch_slot_bytes(world, max_pods)));
     KGPU_CUDA(h, cudaMemset(h->xch.local, 0xFF, (size_t)max_pods * 8));                                   // the exchange kernel keeps it that way
     KGPU_CUDA(h, cudaMemset(xch_flags(h->xch.base, world, max_pods), 0, kgpu::PEER_MAX_WORLD * 4 + 16));  // flags, ticket, error
