@@ -183,3 +183,19 @@ func (k *handle) preemptBatch(pods []int32, lvl []int32) ([]uint64, []uint32, er
 	}
 	return keys, victims, nil
 }
+
+// preemptPlan: preemptBatch taken in order (kgpu_preempt_plan): each pod sees the GPUs the pods before it take and the
+// GPUs their victims free, and no two pods name the same victim.  Dry run: commit with setFreeMasks / setHolders once
+// the victims are gone.
+func (k *handle) preemptPlan(pods []int32, lvl []int32) ([]uint64, []uint32, error) {
+	keys := make([]uint64, len(pods)/4)
+	victims := make([]uint32, len(keys))
+	if len(keys) == 0 {
+		return keys, victims, nil
+	}
+	if rc := C.kgpu_preempt_plan(k.h, (*C.int32_t)(unsafe.Pointer(&pods[0])), (*C.int32_t)(unsafe.Pointer(&lvl[0])),
+		C.int64_t(len(keys)), (*C.uint64_t)(unsafe.Pointer(&keys[0])), (*C.uint32_t)(unsafe.Pointer(&victims[0]))); rc != C.KGPU_OK {
+		return nil, nil, k.err("kgpu_preempt_plan")
+	}
+	return keys, victims, nil
+}

@@ -225,6 +225,26 @@ int kgpu_upload_holders(kgpu_t *h, const int32_t *holders, int64_t n);
 int kgpu_set_holders(kgpu_t *h, const int64_t *idx, const int32_t *holders, int64_t n);
 int kgpu_preempt_batch(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_t P, uint64_t *out_keys,
                        uint32_t *out_victims);
+/* kgpu_preempt_plan: the conflict-free counterpart of kgpu_preempt_batch, as kgpu_place_batch_ex(KGPU_PLACE_DRY_RUN)
+ * is of kgpu_score_batch.  Arguments, output format and validation as for kgpu_preempt_batch.  A working state (F, H)
+ * starts as the handle's free masks and holder table (all -1 if none was uploaded), and the pods are taken IN ORDER:
+ * pod p gets what kgpu_preempt_batch would give it alone on (F, H); if it fits on node n with GPUs S and victims V,
+ * then with R = the non-free GPUs of n whose owner is in V,  F[n] = (F[n] | R) & ~S  (the victims' GPUs that p does
+ * not take are free for later pods) and H[n][g] = -1 for every g in S | R.  Consequences:
+ *   - a pod of the batch is never a victim: GPUs the batch takes are marked -1, so a later pod of a higher level
+ *     cannot evict an earlier one (as in kube-scheduler, where nominated pods are not preemption victims) -- pass the
+ *     pods in priority order;
+ *   - victim bits name owners of the holder table as it was at the call (nothing is renumbered or added);
+ *   - the victim sets of different pods are disjoint, and so are the GPU sets of pods on one node;
+ *   - P = 1 equals kgpu_preempt_batch; without a holder table, or with every lvl 0, the keys equal
+ *     kgpu_place_batch_ex(KGPU_PLACE_DRY_RUN) and every victim mask is 0.
+ * DRY RUN ONLY: the handle's free masks, holder table and caches are untouched.  Victims terminate asynchronously,
+ * so a plan is committed by the caller, with kgpu_set_free_masks and kgpu_set_holders, once they are gone.
+ * Limits (KGPU_ERR_INVALID, checked before anything runs; pods with k outside 0..8 do not count): at most 7 distinct
+ * positive min_mem_mib values, and at most 32 distinct (level, min_mem_mib) pairs among the pods with level > 0.
+ * Single-device handles only (KGPU_ERR_STATE otherwise).  Host buffers, synchronous. */
+int kgpu_preempt_plan(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_t P, uint64_t *out_keys,
+                      uint32_t *out_victims);
 /* Copy the current free masks (n = kgpu_num_nodes entries) back to the host. */
 int kgpu_get_free_masks(kgpu_t *h, int32_t *out_free_mask, int64_t n);
 

@@ -576,6 +576,11 @@ std::string NvidiaGPUScheduler::PreemptBatch(const std::vector<const types::PodI
     return runBatch(pods, out, BatchMode::Preempt, victims);
 }
 
+std::string NvidiaGPUScheduler::PlanPreemption(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
+                                               std::vector<std::vector<std::string>> *victims) {
+    return runBatch(pods, out, BatchMode::PreemptPlan, victims);
+}
+
 // Holder rows from the committed placements: on each node the pods holding GPUs, in name order, are owners 0, 1, ...;
 // a GPU gets level << 3 | owner of the pod that holds it, -1 if no committed placement accounts for it.  Pushed for the
 // nodes changed since the last push (kgpu_set_holders), or all of them after a re-upload reset the table.
@@ -674,12 +679,14 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     std::vector<uint64_t> dev(P, KGPU_NO_FIT);
     std::vector<uint32_t> owners(P, 0);
     std::vector<int32_t> lvl(P, 0);
-    if (mode == BatchMode::Preempt) {
+    const bool preempt = mode == BatchMode::Preempt || mode == BatchMode::PreemptPlan;
+    if (preempt) {
         for (size_t i = 0; i < P; i++) lvl[i] = levelOf(*pods[order[i]]);
         err = pushHolders();
         if (!err.empty()) return err;
     }
     const int rc = mode == BatchMode::Preempt  ? kgpu_preempt_batch(handle_, req.data(), lvl.data(), (int64_t)P, dev.data(), owners.data())
+                   : mode == BatchMode::PreemptPlan ? kgpu_preempt_plan(handle_, req.data(), lvl.data(), (int64_t)P, dev.data(), owners.data())
                    : mode == BatchMode::Snapshot ? kgpu_score_batch(handle_, req.data(), (int64_t)P, dev.data())
                                                : kgpu_place_batch_gang(handle_, req.data(), gang.empty() ? nullptr : gang.data(),
                                                                        (int64_t)P, dev.data(),
@@ -703,13 +710,13 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
                 pl.committed = true;
                 holdersChanged_.insert(pl.nodeName);
             }
-            if (mode == BatchMode::Preempt) {                // order == identity: gangs are not reordered here
+            if (preempt) {                                   // order == identity: gangs are not reordered here
                 const NodeRecord &rec = nodes_[pl.nodeName];
                 for (int o = 0; o < 8; o++)
                     if (((owners[p] >> o) & 1u) && (size_t)o < rec.owners.size()) (*victims)[p].push_back(rec.owners[(size_t)o]);
             }
         }
-        if (mode == BatchMode::Preempt) continue;            // a proposal that needs evictions first: not remembered
+        if (preempt) continue;                               // a proposal that needs evictions first: not remembered
         if (!pods[p]->Name.empty()) lastPlacement_[pods[p]->Name] = pl;
     }
     return "";

@@ -203,6 +203,13 @@ public:
     // may name the same victims, and gang ids are ignored.
     std::string PreemptBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
                              std::vector<std::vector<std::string>> *victims);
+    // The conflict-free counterpart of PreemptBatch, as ProposeBatch is of ScoreBatch (kgpu_preempt_plan): pods are
+    // taken in the caller's order, each on the state the pods before it leave -- their GPUs taken, their victims' GPUs
+    // free, neither evictable again -- so no two pods name the same victim or GPU.  Pass pods in priority order.  Like
+    // PreemptBatch, nothing is evicted, taken or remembered and gang ids are ignored: commit a plan with
+    // TakePodResources / ReturnPodResources once the victims are gone.
+    std::string PlanPreemption(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
+                               std::vector<std::vector<std::string>> *victims);
     std::string LastError() const { return lastError_; }
     const TreeCache &cache() const { return cache_; }
     bool hasDevice() const { return handle_ != nullptr; }
@@ -227,7 +234,7 @@ private:
     std::string syncNode(const NodeRecord &rec);
     std::string flushNodes();
     std::string scoreOne(const NodeRecord &rec, int k, int32_t minMemMiB, uint32_t *nodeKey);
-    enum class BatchMode { Snapshot, Sequential, DryRun, Preempt };
+    enum class BatchMode { Snapshot, Sequential, DryRun, Preempt, PreemptPlan };
     std::string runBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out, BatchMode mode,
                          std::vector<std::vector<std::string>> *victims = nullptr);
     const NodeRecord *recordOf(const types::NodeInfo *nodeInfo) const;

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <chrono>
 #include <cstdarg>
 #include <cstdio>
@@ -19,6 +20,7 @@
 #include "multi_device.h"
 #include "place_sequential.cuh"
 #include "preempt.cuh"
+#include "preempt_plan.cuh"
 #include "sparse_work.h"
 #include "peer_exchange.cuh"
 #include "score_pairs.cuh"
@@ -72,6 +74,12 @@ struct kgpu_shard {
     kgpu::DeviceBuffer<unsigned long long> d_pkey;
     kgpu::DeviceBuffer<uint32_t> d_victims;
     kgpu::DeviceBuffer<int> d_pcnt;
+    kgpu::DeviceBuffer<int32_t> d_plan_free;   // kgpu_preempt_plan: working copies of the free masks [n]
+    kgpu::DeviceBuffer<int32_t> d_plan_hold;   //   and of the holder table [n][8],
+    kgpu::DeviceBuffer<int4> d_plan_cols;      //   the batch's columns {k, level, min_mem, 0}, each pod's column [P],
+    kgpu::DeviceBuffer<int32_t> d_plan_pcol;
+    kgpu::DeviceBuffer<unsigned long long> d_plan_nodekey;   //   per-column node keys [cols][Npad]
+    kgpu::DeviceBuffer<unsigned long long> d_plan_tilekey;   //   and their tile minima [cols][T]
     int64_t class_count[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     int64_t n_slots = 0;
     int64_t n = 0;
@@ -1039,6 +1047,100 @@ int kgpu_preempt_batch(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64
         kgpu::preempt_finalize<<<pb, 256, 0, s.stream>>>(s.d_pkey, s.d_pidx, s.d_pcnt, s.d_free, s.d_hold, s.node_id_base,
                                                          s.d_keys, s.d_victims);
         h->launches += 3;
+        KGPU_CUDA(h, cudaGetLastError());
+    }
+    KGPU_CUDA(h, cudaEventRecord(s.ev1, s.stream));
+    KGPU_CUDA(h, cudaMemcpyAsync(out_keys, s.d_keys, (size_t)P * 8, cudaMemcpyDeviceToHost, s.stream));
+    KGPU_CUDA(h, cudaMemcpyAsync(out_victims, s.d_victims, (size_t)P * 4, cudaMemcpyDeviceToHost, s.stream));
+    KGPU_CUDA(h, cudaStreamSynchronize(s.stream));
+    float ms = 0.f;
+    KGPU_CUDA(h, cudaEventElapsedTime(&ms, s.ev0, s.ev1));
+    h->last_kernel_ms = ms;
+    return KGPU_OK;
+}
+
+int kgpu_preempt_plan(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_t P, uint64_t *out_keys,
+                      uint32_t *out_victims) {
+    if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: NULL handle");
+    std::lock_guard<std::mutex> g(h->mu);
+    if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_preempt_plan: needs a single-device handle");
+    if (P < 0 || (P > 0 && (!pods || !lvl || !out_keys || !out_victims)))
+        return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: bad arguments");
+    for (int64_t p = 0; p < P; p++)
+        if (lvl[p] < 0 || lvl[p] > 15) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: lvl[%lld] = %d outside 0..15", (long long)p, lvl[p]);
+    if (P == 0) return KGPU_OK;
+    if (P > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: more than 2^31 pods");
+    // The batch's columns: distinct (k, level, min_mem) with k in 1..8, sorted (k first, so warps stay on one k).
+    std::vector<std::array<int32_t, 3>> trip;
+    std::vector<int32_t> mems;
+    std::vector<std::pair<int32_t, int32_t>> views;      // (level, min_mem) with level > 0
+    for (int64_t p = 0; p < P; p++) {
+        const int32_t k = pods[4 * p], need = std::max<int32_t>(0, pods[4 * p + 3]);
+        if (k < 0 || k > 8) continue;
+        if (need > 0) mems.push_back(need);
+        if (lvl[p] > 0) views.push_back({lvl[p], need});
+        if (k > 0) trip.push_back({k, lvl[p], need});
+    }
+    std::sort(trip.begin(), trip.end());
+    trip.erase(std::unique(trip.begin(), trip.end()), trip.end());
+    std::sort(mems.begin(), mems.end());
+    mems.erase(std::unique(mems.begin(), mems.end()), mems.end());
+    std::sort(views.begin(), views.end());
+    views.erase(std::unique(views.begin(), views.end()), views.end());
+    if (mems.size() > (size_t)kgpu::PLACE_MAX_VIEWS - 1)
+        return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: more than %d distinct min_mem values in one batch", kgpu::PLACE_MAX_VIEWS - 1);
+    if (views.size() > 32)
+        return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: more than 32 distinct (level > 0, min_mem) pairs in one batch");
+    const int ncol = (int)trip.size();           // <= 8 k x (8 level-0 + 32 other views) = PLAN_MAX_COLS
+    std::vector<int4> cols((size_t)ncol);
+    for (int c = 0; c < ncol; c++) cols[(size_t)c] = make_int4(trip[(size_t)c][0], trip[(size_t)c][1], trip[(size_t)c][2], 0);
+    std::vector<int32_t> pcol((size_t)P, -1);
+    for (int64_t p = 0; p < P; p++) {
+        const int32_t k = pods[4 * p];
+        if (k < 1 || k > 8) continue;
+        const std::array<int32_t, 3> t = {k, lvl[p], std::max<int32_t>(0, pods[4 * p + 3])};
+        pcol[(size_t)p] = (int32_t)(std::lower_bound(trip.begin(), trip.end(), t) - trip.begin());
+    }
+    kgpu_shard &s = h->shards[0];
+    if (s.n > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: too many nodes for the key's node field");
+    int rc = reserve_pods(h, s, P);
+    if (rc != KGPU_OK) return rc;
+    const int64_t cap = pod_headroom(P);
+    KGPU_CUDA(h, s.d_victims.reserve(P, cap));
+    KGPU_CUDA(h, s.d_plan_pcol.reserve(P, cap));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_pods, pods, (size_t)P * 16, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_plan_pcol, pcol.data(), (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, cudaEventRecord(s.ev0, s.stream));
+    if (s.n == 0) {
+        KGPU_CUDA(h, cudaMemsetAsync(s.d_keys, 0xFF, (size_t)P * 8, s.stream));
+        KGPU_CUDA(h, cudaMemsetAsync(s.d_victims, 0, (size_t)P * 4, s.stream));
+    } else {
+        const int64_t T = (s.n + kgpu::PLAN_TILE - 1) / kgpu::PLAN_TILE, Npad = T * kgpu::PLAN_TILE;
+        // the working state (F, H): the handle's masks and holder table are never written
+        KGPU_CUDA(h, s.d_plan_free.reserve(s.n));
+        KGPU_CUDA(h, s.d_plan_hold.reserve(8 * s.n));
+        KGPU_CUDA(h, cudaMemcpyAsync(s.d_plan_free, s.d_free, (size_t)s.n * 4, cudaMemcpyDeviceToDevice, s.stream));
+        if (s.has_hold) KGPU_CUDA(h, cudaMemcpyAsync(s.d_plan_hold, s.d_hold, (size_t)s.n * 32, cudaMemcpyDeviceToDevice, s.stream));
+        else KGPU_CUDA(h, cudaMemsetAsync(s.d_plan_hold, 0xFF, (size_t)s.n * 32, s.stream));
+        kgpu::Weights W;
+        memcpy(W.w, h->W, sizeof W.w);
+        if (ncol > 0) {
+            KGPU_CUDA(h, s.d_plan_cols.reserve(ncol));
+            KGPU_CUDA(h, s.d_plan_nodekey.reserve(ncol * Npad));
+            KGPU_CUDA(h, s.d_plan_tilekey.reserve(ncol * T));
+            KGPU_CUDA(h, cudaMemcpyAsync(s.d_plan_cols, cols.data(), (size_t)ncol * 16, cudaMemcpyHostToDevice, s.stream));
+            const unsigned groups = (unsigned)((ncol + kgpu::PLAN_INIT_COLS - 1) / kgpu::PLAN_INIT_COLS);
+            kgpu::plan_init<<<dim3((unsigned)T, groups), kgpu::PLAN_TILE, 0, s.stream>>>(
+                reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_plan_free, reinterpret_cast<const int4 *>(s.d_mem.get()),
+                reinterpret_cast<const int4 *>(s.d_plan_hold.get()), s.n, Npad, T, s.d_plan_cols, ncol, W, PC, s.d_plan_nodekey,
+                s.d_plan_tilekey);
+            h->launches++;
+        }
+        kgpu::plan_sequential<<<1, kgpu::PLAN_THREADS, 0, s.stream>>>(
+            reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_plan_free, reinterpret_cast<const int4 *>(s.d_mem.get()),
+            s.d_plan_hold, s.n, Npad, T, s.node_id_base, reinterpret_cast<const int4 *>(s.d_pods.get()), s.d_plan_pcol, P,
+            s.d_plan_cols, ncol, W, PC, s.d_plan_nodekey, s.d_plan_tilekey, s.d_keys, s.d_victims);
+        h->launches++;
         KGPU_CUDA(h, cudaGetLastError());
     }
     KGPU_CUDA(h, cudaEventRecord(s.ev1, s.stream));

@@ -198,6 +198,20 @@ class Scorer:
                                                victims.ctypes.data))
         return keys, victims
 
+    def preempt_plan(self, pods, lvl):
+        """(keys uint64[P], victims uint32[P]) as preempt_batch, but conflict-free: pods are taken in order, each on the
+        state the pods before it leave (their GPUs taken, their victims' GPUs free, neither evictable again).  Victim
+        sets are disjoint.  Dry run: the handle's masks and holder table are untouched.  Pass pods in priority order."""
+        pods, lvl = _i32(pods), _i32(lvl)
+        P = pods.size // 4
+        if lvl.size != P:
+            raise ValueError("lvl must hold one level per pod")
+        keys = np.empty(P, dtype=np.uint64)
+        victims = np.empty(P, dtype=np.uint32)
+        self._check(self._L.kgpu_preempt_plan(self._h, pods.ctypes.data, lvl.ctypes.data, P, keys.ctypes.data,
+                                              victims.ctypes.data))
+        return keys, victims
+
     def get_free_masks(self) -> np.ndarray:
         out = np.empty(self.num_nodes, dtype=np.int32)
         self._check(self._L.kgpu_get_free_masks(self._h, out.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), out.shape[0]))
