@@ -199,3 +199,19 @@ func (k *handle) preemptPlan(pods []int32, lvl []int32) ([]uint64, []uint32, err
 	}
 	return keys, victims, nil
 }
+
+// preemptPlanGang: preemptPlan with gang ids (kgpu_preempt_plan_gang, ids as for placeBatch): a gang's members
+// evict and take all together or not at all, and a failed gang's would-be victims stay available to later pods.
+func (k *handle) preemptPlanGang(pods []int32, lvl []int32, gang []int32) ([]uint64, []uint32, error) {
+	keys := make([]uint64, len(pods)/4)
+	victims := make([]uint32, len(keys))
+	if len(keys) == 0 {
+		return keys, victims, nil
+	}
+	if rc := C.kgpu_preempt_plan_gang(k.h, (*C.int32_t)(unsafe.Pointer(&pods[0])), (*C.int32_t)(unsafe.Pointer(&lvl[0])),
+		(*C.int32_t)(unsafe.Pointer(&gang[0])), C.int64_t(len(keys)), (*C.uint64_t)(unsafe.Pointer(&keys[0])),
+		(*C.uint32_t)(unsafe.Pointer(&victims[0]))); rc != C.KGPU_OK {
+		return nil, nil, k.err("kgpu_preempt_plan_gang")
+	}
+	return keys, victims, nil
+}

@@ -245,6 +245,21 @@ int kgpu_preempt_batch(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64
  * Single-device handles only (KGPU_ERR_STATE otherwise).  Host buffers, synchronous. */
 int kgpu_preempt_plan(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_t P, uint64_t *out_keys,
                       uint32_t *out_victims);
+/* kgpu_preempt_plan with gangs: the members of a gang (a multi-pod training job) evict their victims and take their
+ * GPUs all together, or not at all.  gang[P] as for kgpu_place_batch_gang: 0 = the pod is on its own, a GANG is a
+ * maximal run of consecutive pods with the same nonzero id, and an id that appears in two separate runs is
+ * KGPU_ERR_INVALID (checked before anything runs).  Pods are taken in order on (F, H) exactly as by kgpu_preempt_plan.
+ * When a member gets no candidate, or asks for k outside 0..8:
+ *   - the members of its gang taken before it are undone, last first: each member's node gets back the free mask and
+ *     holder row it had just before that member's update, so the victims they named are running pods again and later
+ *     pods of the batch may name them;
+ *   - the members after it are not tried;
+ *   - every member of the gang gets KGPU_NO_FIT and victims 0.
+ * The result equals kgpu_preempt_plan on the batch with every failed gang deleted.  Members may differ in k, level and
+ * min_mem_mib; a k = 0 member fits and takes nothing.  gang == NULL is kgpu_preempt_plan.  Dry run only, limits,
+ * single-device handles, host buffers and synchronous, as for kgpu_preempt_plan. */
+int kgpu_preempt_plan_gang(kgpu_t *h, const int32_t *pods, const int32_t *lvl, const int32_t *gang, int64_t P,
+                           uint64_t *out_keys, uint32_t *out_victims);
 /* Copy the current free masks (n = kgpu_num_nodes entries) back to the host. */
 int kgpu_get_free_masks(kgpu_t *h, int32_t *out_free_mask, int64_t n);
 

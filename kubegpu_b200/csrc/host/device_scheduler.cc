@@ -581,6 +581,11 @@ std::string NvidiaGPUScheduler::PlanPreemption(const std::vector<const types::Po
     return runBatch(pods, out, BatchMode::PreemptPlan, victims);
 }
 
+std::string NvidiaGPUScheduler::PlanGangPreemption(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
+                                                   std::vector<std::vector<std::string>> *victims) {
+    return runBatch(pods, out, BatchMode::PreemptGangPlan, victims);
+}
+
 // Holder rows from the committed placements: on each node the pods holding GPUs, in name order, are owners 0, 1, ...;
 // a GPU gets level << 3 | owner of the pod that holds it, -1 if no committed placement accounts for it.  Pushed for the
 // nodes changed since the last push (kgpu_set_holders), or all of them after a re-upload reset the table.
@@ -628,13 +633,13 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     std::string err = flushNodes();
     if (!err.empty()) return err;
     const size_t P = pods.size();
-    // Gangs (sequential modes only): the device takes a gang as one run of consecutive pods with an int32 id, so the
+    // Gangs (sequential modes and gang plans only): the device takes a gang as one run of consecutive pods with an int32 id, so the
     // ids are renumbered 1, 2, ... in order of first appearance (no truncation can merge two gangs) and each member
     // moves up to its gang's first member.  order[i] = the caller's index of the pod at device position i.
     std::vector<size_t> order(P);
     std::vector<int32_t> gang;
     for (size_t p = 0; p < P; p++) order[p] = p;
-    if (mode == BatchMode::Sequential || mode == BatchMode::DryRun) {
+    if (mode == BatchMode::Sequential || mode == BatchMode::DryRun || mode == BatchMode::PreemptGangPlan) {
         std::map<int64_t, int32_t> dense;
         std::vector<std::vector<size_t>> members;
         std::vector<int32_t> gangOf(P, 0);
@@ -679,7 +684,7 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     std::vector<uint64_t> dev(P, KGPU_NO_FIT);
     std::vector<uint32_t> owners(P, 0);
     std::vector<int32_t> lvl(P, 0);
-    const bool preempt = mode == BatchMode::Preempt || mode == BatchMode::PreemptPlan;
+    const bool preempt = mode == BatchMode::Preempt || mode == BatchMode::PreemptPlan || mode == BatchMode::PreemptGangPlan;
     if (preempt) {
         for (size_t i = 0; i < P; i++) lvl[i] = levelOf(*pods[order[i]]);
         err = pushHolders();
@@ -687,13 +692,20 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     }
     const int rc = mode == BatchMode::Preempt  ? kgpu_preempt_batch(handle_, req.data(), lvl.data(), (int64_t)P, dev.data(), owners.data())
                    : mode == BatchMode::PreemptPlan ? kgpu_preempt_plan(handle_, req.data(), lvl.data(), (int64_t)P, dev.data(), owners.data())
+                   : mode == BatchMode::PreemptGangPlan
+                       ? kgpu_preempt_plan_gang(handle_, req.data(), lvl.data(), gang.empty() ? nullptr : gang.data(), (int64_t)P,
+                                                dev.data(), owners.data())
                    : mode == BatchMode::Snapshot ? kgpu_score_batch(handle_, req.data(), (int64_t)P, dev.data())
                                                : kgpu_place_batch_gang(handle_, req.data(), gang.empty() ? nullptr : gang.data(),
                                                                        (int64_t)P, dev.data(),
                                                                        mode == BatchMode::DryRun ? KGPU_PLACE_DRY_RUN : 0);
     if (rc != KGPU_OK) return lastError_ = kgpu_last_error(handle_);
     std::vector<uint64_t> keys(P, KGPU_NO_FIT);           // back in the caller's order
-    for (size_t i = 0; i < P; i++) keys[order[i]] = dev[i];
+    std::vector<uint32_t> vic(P, 0);
+    for (size_t i = 0; i < P; i++) {
+        keys[order[i]] = dev[i];
+        vic[order[i]] = owners[i];
+    }
     out->assign(P, Placement());
     if (victims) victims->assign(P, {});
     for (size_t p = 0; p < P; p++) {
@@ -710,10 +722,10 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
                 pl.committed = true;
                 holdersChanged_.insert(pl.nodeName);
             }
-            if (preempt) {                                   // order == identity: gangs are not reordered here
+            if (preempt) {
                 const NodeRecord &rec = nodes_[pl.nodeName];
                 for (int o = 0; o < 8; o++)
-                    if (((owners[p] >> o) & 1u) && (size_t)o < rec.owners.size()) (*victims)[p].push_back(rec.owners[(size_t)o]);
+                    if (((vic[p] >> o) & 1u) && (size_t)o < rec.owners.size()) (*victims)[p].push_back(rec.owners[(size_t)o]);
             }
         }
         if (preempt) continue;                               // a proposal that needs evictions first: not remembered

@@ -210,6 +210,12 @@ public:
     // TakePodResources / ReturnPodResources once the victims are gone.
     std::string PlanPreemption(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
                                std::vector<std::vector<std::string>> *victims);
+    // PlanPreemption with gangs (GPUGangID, kgpu_preempt_plan_gang): members are moved up to their gang's first member
+    // as in PlaceBatch, and a gang evicts and takes all together or not at all.  If one member cannot be placed, the
+    // whole gang gets fits = false and no victims, and the pods after it see the victims its other members would have
+    // named as running pods again.  `out` and `victims` are in the caller's order.
+    std::string PlanGangPreemption(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
+                                   std::vector<std::vector<std::string>> *victims);
     std::string LastError() const { return lastError_; }
     const TreeCache &cache() const { return cache_; }
     bool hasDevice() const { return handle_ != nullptr; }
@@ -234,7 +240,7 @@ private:
     std::string syncNode(const NodeRecord &rec);
     std::string flushNodes();
     std::string scoreOne(const NodeRecord &rec, int k, int32_t minMemMiB, uint32_t *nodeKey);
-    enum class BatchMode { Snapshot, Sequential, DryRun, Preempt, PreemptPlan };
+    enum class BatchMode { Snapshot, Sequential, DryRun, Preempt, PreemptPlan, PreemptGangPlan };
     std::string runBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out, BatchMode mode,
                          std::vector<std::vector<std::string>> *victims = nullptr);
     const NodeRecord *recordOf(const types::NodeInfo *nodeInfo) const;

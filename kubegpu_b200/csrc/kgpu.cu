@@ -80,12 +80,13 @@ struct kgpu_shard {
     kgpu::DeviceBuffer<int32_t> d_plan_pcol;
     kgpu::DeviceBuffer<unsigned long long> d_plan_nodekey;   //   per-column node keys [cols][Npad]
     kgpu::DeviceBuffer<unsigned long long> d_plan_tilekey;   //   and their tile minima [cols][T]
+    kgpu::DeviceBuffer<int4> d_plan_pre;       // kgpu_preempt_plan_gang: each placed member's pre-image {F, H row} [P]
     int64_t class_count[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     int64_t n_slots = 0;
     int64_t n = 0;
     int64_t node_id_base = 0;
     kgpu::DeviceBuffer<int32_t> d_pods;       // [P][4]
-    kgpu::DeviceBuffer<int32_t> d_gang;       // [P] kgpu_place_batch_gang: gang id per pod
+    kgpu::DeviceBuffer<int32_t> d_gang;       // [P] kgpu_place_batch_gang / kgpu_preempt_plan_gang: gang id per pod
     kgpu::DeviceBuffer<unsigned long long> d_keys;     // [P]
     kgpu::DeviceBuffer<unsigned long long> d_gather;   // [ndev][P] (multi-device only)
     kgpu::DeviceBuffer<unsigned long long> d_bestk;    // [9] memo variant
@@ -814,6 +815,19 @@ int kgpu_score_batch(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out_ke
     return KGPU_OK;
 }
 
+namespace {
+// A gang is ONE run of consecutive pods: the kernels only look at neighbours, so an id in two separate runs is refused.
+int check_gang_runs(kgpu_ctx *h, const char *fn, const int32_t *gang, int64_t P) {
+    std::unordered_set<int32_t> seen;
+    for (int64_t p = 0; p < P; p++) {
+        if (gang[p] == 0 || (p > 0 && gang[p - 1] == gang[p])) continue;
+        if (!seen.insert(gang[p]).second)
+            return fail(h, KGPU_ERR_INVALID, "%s: gang id %d appears in two separate runs (again at pod %lld)", fn, gang[p], (long long)p);
+    }
+    return KGPU_OK;
+}
+}  // namespace
+
 int kgpu_place_batch(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out_keys) {
     return kgpu_place_batch_ex(h, pods, P, out_keys, 0);
 }
@@ -828,14 +842,9 @@ int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, i
     if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_place_batch: needs a single-device handle");
     if (P < 0 || (P > 0 && (!pods || !out_keys))) return fail(h, KGPU_ERR_INVALID, "kgpu_place_batch: bad arguments");
     if (P == 0) return KGPU_OK;
-    if (gang) {                            // a gang is ONE run of consecutive pods: the kernel only looks at neighbours
-        std::unordered_set<int32_t> seen;
-        for (int64_t p = 0; p < P; p++) {
-            if (gang[p] == 0 || (p > 0 && gang[p - 1] == gang[p])) continue;
-            if (!seen.insert(gang[p]).second)
-                return fail(h, KGPU_ERR_INVALID, "kgpu_place_batch_gang: gang id %d appears in two separate runs (again at pod %lld)",
-                            gang[p], (long long)p);
-        }
+    if (gang) {
+        const int rc = check_gang_runs(h, "kgpu_place_batch_gang", gang, P);
+        if (rc != KGPU_OK) return rc;
     }
     // the batch's distinct memory requirements are the views the sequential kernels keep tables for
     kgpu::PlaceViews views;
@@ -1059,18 +1068,14 @@ int kgpu_preempt_batch(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64
     return KGPU_OK;
 }
 
-int kgpu_preempt_plan(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_t P, uint64_t *out_keys,
-                      uint32_t *out_victims) {
-    if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: NULL handle");
-    std::lock_guard<std::mutex> g(h->mu);
-    if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_preempt_plan: needs a single-device handle");
-    if (P < 0 || (P > 0 && (!pods || !lvl || !out_keys || !out_victims)))
-        return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: bad arguments");
+namespace {
+// kgpu_preempt_plan[_gang]: the batch's checks and its columns, the distinct (k, level, min_mem) with k in 1..8, sorted
+// (k first, so warps stay on one k); pcol[p] = pod p's column, -1 for k outside 1..8.
+int plan_columns(kgpu_ctx *h, const char *fn, const int32_t *pods, const int32_t *lvl, int64_t P, std::vector<int4> &cols,
+                 std::vector<int32_t> &pcol) {
     for (int64_t p = 0; p < P; p++)
-        if (lvl[p] < 0 || lvl[p] > 15) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: lvl[%lld] = %d outside 0..15", (long long)p, lvl[p]);
-    if (P == 0) return KGPU_OK;
-    if (P > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: more than 2^31 pods");
-    // The batch's columns: distinct (k, level, min_mem) with k in 1..8, sorted (k first, so warps stay on one k).
+        if (lvl[p] < 0 || lvl[p] > 15) return fail(h, KGPU_ERR_INVALID, "%s: lvl[%lld] = %d outside 0..15", fn, (long long)p, lvl[p]);
+    if (P > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "%s: more than 2^31 pods", fn);
     std::vector<std::array<int32_t, 3>> trip;
     std::vector<int32_t> mems;
     std::vector<std::pair<int32_t, int32_t>> views;      // (level, min_mem) with level > 0
@@ -1088,35 +1093,33 @@ int kgpu_preempt_plan(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_
     std::sort(views.begin(), views.end());
     views.erase(std::unique(views.begin(), views.end()), views.end());
     if (mems.size() > (size_t)kgpu::PLACE_MAX_VIEWS - 1)
-        return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: more than %d distinct min_mem values in one batch", kgpu::PLACE_MAX_VIEWS - 1);
-    if (views.size() > 32)
-        return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: more than 32 distinct (level > 0, min_mem) pairs in one batch");
+        return fail(h, KGPU_ERR_INVALID, "%s: more than %d distinct min_mem values in one batch", fn, kgpu::PLACE_MAX_VIEWS - 1);
+    if (views.size() > 32) return fail(h, KGPU_ERR_INVALID, "%s: more than 32 distinct (level > 0, min_mem) pairs in one batch", fn);
     const int ncol = (int)trip.size();           // <= 8 k x (8 level-0 + 32 other views) = PLAN_MAX_COLS
-    std::vector<int4> cols((size_t)ncol);
+    cols.resize((size_t)ncol);
     for (int c = 0; c < ncol; c++) cols[(size_t)c] = make_int4(trip[(size_t)c][0], trip[(size_t)c][1], trip[(size_t)c][2], 0);
-    std::vector<int32_t> pcol((size_t)P, -1);
+    pcol.assign((size_t)P, -1);
     for (int64_t p = 0; p < P; p++) {
         const int32_t k = pods[4 * p];
         if (k < 1 || k > 8) continue;
         const std::array<int32_t, 3> t = {k, lvl[p], std::max<int32_t>(0, pods[4 * p + 3])};
         pcol[(size_t)p] = (int32_t)(std::lower_bound(trip.begin(), trip.end(), t) - trip.begin());
     }
-    kgpu_shard &s = h->shards[0];
-    if (s.n > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: too many nodes for the key's node field");
-    int rc = reserve_pods(h, s, P);
-    if (rc != KGPU_OK) return rc;
-    const int64_t cap = pod_headroom(P);
-    KGPU_CUDA(h, s.d_victims.reserve(P, cap));
-    KGPU_CUDA(h, s.d_plan_pcol.reserve(P, cap));
-    KGPU_CUDA(h, cudaMemcpyAsync(s.d_pods, pods, (size_t)P * 16, cudaMemcpyHostToDevice, s.stream));
-    KGPU_CUDA(h, cudaMemcpyAsync(s.d_plan_pcol, pcol.data(), (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
+    if (h->shards[0].n > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "%s: too many nodes for the key's node field", fn);
+    return KGPU_OK;
+}
+
+// The plan's kernels on the working state (F, H), once the batch is on the device (d_pods, d_plan_pcol and, with gangs,
+// d_gang), then the results back to the host.  The handle's masks and holder table are never written.
+int plan_launch(kgpu_ctx *h, kgpu_shard &s, int64_t P, const std::vector<int4> &cols, bool gang, uint64_t *out_keys,
+                uint32_t *out_victims) {
+    const int ncol = (int)cols.size();
     KGPU_CUDA(h, cudaEventRecord(s.ev0, s.stream));
     if (s.n == 0) {
         KGPU_CUDA(h, cudaMemsetAsync(s.d_keys, 0xFF, (size_t)P * 8, s.stream));
         KGPU_CUDA(h, cudaMemsetAsync(s.d_victims, 0, (size_t)P * 4, s.stream));
     } else {
         const int64_t T = (s.n + kgpu::PLAN_TILE - 1) / kgpu::PLAN_TILE, Npad = T * kgpu::PLAN_TILE;
-        // the working state (F, H): the handle's masks and holder table are never written
         KGPU_CUDA(h, s.d_plan_free.reserve(s.n));
         KGPU_CUDA(h, s.d_plan_hold.reserve(8 * s.n));
         KGPU_CUDA(h, cudaMemcpyAsync(s.d_plan_free, s.d_free, (size_t)s.n * 4, cudaMemcpyDeviceToDevice, s.stream));
@@ -1136,10 +1139,16 @@ int kgpu_preempt_plan(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_
                 s.d_plan_tilekey);
             h->launches++;
         }
-        kgpu::plan_sequential<<<1, kgpu::PLAN_THREADS, 0, s.stream>>>(
-            reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_plan_free, reinterpret_cast<const int4 *>(s.d_mem.get()),
-            s.d_plan_hold, s.n, Npad, T, s.node_id_base, reinterpret_cast<const int4 *>(s.d_pods.get()), s.d_plan_pcol, P,
-            s.d_plan_cols, ncol, W, PC, s.d_plan_nodekey, s.d_plan_tilekey, s.d_keys, s.d_victims);
+        if (gang)
+            kgpu::gang_plan_sequential<<<1, kgpu::PLAN_THREADS, 0, s.stream>>>(
+                reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_plan_free, reinterpret_cast<const int4 *>(s.d_mem.get()),
+                s.d_plan_hold, s.n, Npad, T, s.node_id_base, reinterpret_cast<const int4 *>(s.d_pods.get()), s.d_plan_pcol, P,
+                s.d_plan_cols, ncol, W, PC, s.d_plan_nodekey, s.d_plan_tilekey, s.d_keys, s.d_victims, s.d_gang, s.d_plan_pre);
+        else
+            kgpu::plan_sequential<<<1, kgpu::PLAN_THREADS, 0, s.stream>>>(
+                reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_plan_free, reinterpret_cast<const int4 *>(s.d_mem.get()),
+                s.d_plan_hold, s.n, Npad, T, s.node_id_base, reinterpret_cast<const int4 *>(s.d_pods.get()), s.d_plan_pcol, P,
+                s.d_plan_cols, ncol, W, PC, s.d_plan_nodekey, s.d_plan_tilekey, s.d_keys, s.d_victims);
         h->launches++;
         KGPU_CUDA(h, cudaGetLastError());
     }
@@ -1151,6 +1160,59 @@ int kgpu_preempt_plan(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_
     KGPU_CUDA(h, cudaEventElapsedTime(&ms, s.ev0, s.ev1));
     h->last_kernel_ms = ms;
     return KGPU_OK;
+}
+}  // namespace
+
+int kgpu_preempt_plan(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_t P, uint64_t *out_keys,
+                      uint32_t *out_victims) {
+    if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: NULL handle");
+    std::lock_guard<std::mutex> g(h->mu);
+    if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_preempt_plan: needs a single-device handle");
+    if (P < 0 || (P > 0 && (!pods || !lvl || !out_keys || !out_victims)))
+        return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan: bad arguments");
+    if (P == 0) return KGPU_OK;
+    std::vector<int4> cols;
+    std::vector<int32_t> pcol;
+    int rc = plan_columns(h, "kgpu_preempt_plan", pods, lvl, P, cols, pcol);
+    if (rc != KGPU_OK) return rc;
+    kgpu_shard &s = h->shards[0];
+    rc = reserve_pods(h, s, P);
+    if (rc != KGPU_OK) return rc;
+    const int64_t cap = pod_headroom(P);
+    KGPU_CUDA(h, s.d_victims.reserve(P, cap));
+    KGPU_CUDA(h, s.d_plan_pcol.reserve(P, cap));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_pods, pods, (size_t)P * 16, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_plan_pcol, pcol.data(), (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
+    return plan_launch(h, s, P, cols, false, out_keys, out_victims);
+}
+
+int kgpu_preempt_plan_gang(kgpu_t *h, const int32_t *pods, const int32_t *lvl, const int32_t *gang, int64_t P,
+                           uint64_t *out_keys, uint32_t *out_victims) {
+    if (!gang) return kgpu_preempt_plan(h, pods, lvl, P, out_keys, out_victims);
+    if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan_gang: NULL handle");
+    std::lock_guard<std::mutex> g(h->mu);
+    if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_preempt_plan_gang: needs a single-device handle");
+    if (P < 0 || (P > 0 && (!pods || !lvl || !out_keys || !out_victims)))
+        return fail(h, KGPU_ERR_INVALID, "kgpu_preempt_plan_gang: bad arguments");
+    if (P == 0) return KGPU_OK;
+    int rc = check_gang_runs(h, "kgpu_preempt_plan_gang", gang, P);
+    if (rc != KGPU_OK) return rc;
+    std::vector<int4> cols;
+    std::vector<int32_t> pcol;
+    rc = plan_columns(h, "kgpu_preempt_plan_gang", pods, lvl, P, cols, pcol);
+    if (rc != KGPU_OK) return rc;
+    kgpu_shard &s = h->shards[0];
+    rc = reserve_pods(h, s, P);
+    if (rc != KGPU_OK) return rc;
+    const int64_t cap = pod_headroom(P);
+    KGPU_CUDA(h, s.d_victims.reserve(P, cap));
+    KGPU_CUDA(h, s.d_plan_pcol.reserve(P, cap));
+    KGPU_CUDA(h, s.d_gang.reserve(P, cap));
+    KGPU_CUDA(h, s.d_plan_pre.reserve(P, cap));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_pods, pods, (size_t)P * 16, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_plan_pcol, pcol.data(), (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_gang, gang, (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
+    return plan_launch(h, s, P, cols, true, out_keys, out_victims);
 }
 
 int kgpu_get_free_masks(kgpu_t *h, int32_t *out_free_mask, int64_t n) {

@@ -1,4 +1,4 @@
-// preempt_plan.cuh -- K5: preemption plans for a whole batch (kgpu_preempt_plan), sm_90a.
+// preempt_plan.cuh -- K5: preemption plans for a whole batch (kgpu_preempt_plan[_gang]), sm_90a.
 //
 // Definition (include/kgpu.h).  Pods are taken in order on a working copy (F, H) of the free masks and the holder
 // table.  Pod p gets what kgpu_preempt_batch would give it alone on (F, H); if it fits on node n with GPUs S and
@@ -19,6 +19,8 @@
 //                   winner (its key names node and S); one thread applies the update to (F, H) and writes the key and
 //                   the victims; then one thread per column re-runs the class search on the winner's node, and a tile
 //                   minimum is rescanned (warp per column) only where the node held it and its key went up.
+// gang_plan_sequential: plan_sequential with gangs (kgpu_preempt_plan_gang): a failed gang's placed members are undone
+//                   from per-member pre-images of (F[n], H[n]); both kernels share plan_sequential_body<GANG>.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -178,17 +180,76 @@ plan_init(const int4 *__restrict__ topo4, const int32_t *__restrict__ free_mask,
     }
 }
 
+// Steps 3 and 4 of plan_sequential for node n, whose new state the block has staged in sF / sH: every column's key of the
+// node; the tile minimum follows at once where it can (the key went down, or the node did not hold the minimum),
+// otherwise it is rescanned, warp per column, from the 128 node keys of the tile.  Ends with a barrier.
+__device__ __forceinline__ void plan_refresh(int64_t n, const int4 *__restrict__ topo4, const int4 *__restrict__ mem4, int64_t Npad,
+                                             int64_t T, int ncol, PipeConsts pc, unsigned long long *nodekey,
+                                             unsigned long long *tilekey, const int32_t *sW, const int4 *sCol, const int32_t &sF,
+                                             const int32_t *sH, int32_t *sResc, int &sNresc) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int64_t tile = n / PLAN_TILE;
+    // 3. every column's key of the node under the new state
+    if (tid < ncol) {
+        PairCosts C;
+        plan_pair_costs(topo4, n, true, sW, C);
+        const uint32_t F = (uint32_t)sF & 0xFFu;
+        int32_t mem[8], h[8];
+        const int4 m0 = __ldg(mem4 + n * 2), m1 = __ldg(mem4 + n * 2 + 1);
+        mem[0] = m0.x; mem[1] = m0.y; mem[2] = m0.z; mem[3] = m0.w;
+        mem[4] = m1.x; mem[5] = m1.y; mem[6] = m1.z; mem[7] = m1.w;
+#pragma unroll
+        for (int g = 0; g < 8; g++) h[g] = sH[g];
+        uint64_t gm;
+        uint32_t lvp;
+        plan_owners(h, F, gm, lvp);
+        const unsigned long long old = tilekey[(int64_t)tid * T + tile];
+        const unsigned long long key = plan_node_key(C, pc, F, gm, lvp, mem, sCol[tid], n);
+        nodekey[(int64_t)tid * Npad + n] = key;
+        if (key < old) tilekey[(int64_t)tid * T + tile] = key;
+        else if (key != old && old != ~0ull && (int64_t)((old >> 8) & 0x7FFFFFFFull) == n) sResc[atomicAdd(&sNresc, 1)] = tid;
+    }
+    __syncthreads();
+    // 4. rescans: warp per column, the 128 node keys of the tile
+    const int nr = sNresc;
+    for (int j = warp; j < nr; j += PLAN_WARPS) {
+        const int cc = sResc[j];
+        const unsigned long long *row = nodekey + (int64_t)cc * Npad + tile * PLAN_TILE;
+        unsigned long long m = ~0ull;
+#pragma unroll
+        for (int q = 0; q < PLAN_TILE / 32; q++) m = min(m, row[lane + 32 * q]);
+        m = warp_min_u64_redux(m);
+        if (lane == 0) tilekey[(int64_t)cc * T + tile] = m;
+    }
+    __syncthreads();
+}
+
 // One block of PLAN_THREADS.  pcol[p] = pod p's column, -1 for k outside 1..8 (k == 0 fits on the first node and takes
 // nothing).  free_mask and hold are the working copies (F, H) and are updated in place; keys[p] and victims[p] are
 // written for every pod.
-__global__ void __launch_bounds__(PLAN_THREADS, 1)
-plan_sequential(const int4 *__restrict__ topo4, int32_t *free_mask, const int4 *__restrict__ mem4, int32_t *hold, int64_t N,
-                int64_t Npad, int64_t T, int64_t node_id_base, const int4 *__restrict__ pods4, const int32_t *__restrict__ pcol,
-                int64_t P, const int4 *__restrict__ cols, int ncol, Weights W, PipeConsts pc, unsigned long long *nodekey,
-                unsigned long long *tilekey, unsigned long long *__restrict__ keys, uint32_t *__restrict__ victims) {
+//
+// Gangs (GANG = true): a maximal run of consecutive pods with the same nonzero id gang[p] evicts and takes all or
+// nothing.  The thread that applies a member's update first stores the node's state before it, (F[n], H[n]), in pre[p]
+// ({F, holder bytes 0..3, holder bytes 4..7, 0}).  When a member misses (no candidate, or k outside 0..8), the members
+// placed before it are undone, last first: their keys are read back from keys[] (k == 0 members took nothing), (F[n],
+// H[n]) is restored from pre[], and steps 3 and 4 refresh the node as after a placement.  An undo can raise a key on the
+// node that holds its tile's minimum (a placement frees a victim's other GPUs), so the rescan is needed here too.  Keys
+// and pre-images are in global memory, so a gang may cross a staging chunk.  Members after the miss are not tried, and
+// every member gets NO_FIT and victims 0.  The host guarantees that no id appears in two separate runs.  GANG = false
+// is the plain kernel, with no gang bookkeeping on its chain.
+// W by reference: a by-value copy changes the plain kernel's code.
+template <bool GANG>
+__device__ __forceinline__ void plan_sequential_body(const int4 *__restrict__ topo4, int32_t *free_mask, const int4 *__restrict__ mem4,
+                                                     int32_t *hold, int64_t N, int64_t Npad, int64_t T, int64_t node_id_base,
+                                                     const int4 *__restrict__ pods4, const int32_t *__restrict__ pcol, int64_t P,
+                                                     const int4 *__restrict__ cols, int ncol, const Weights &W, PipeConsts pc,
+                                                     unsigned long long *nodekey, unsigned long long *tilekey,
+                                                     unsigned long long *__restrict__ keys, uint32_t *__restrict__ victims,
+                                                     const int32_t *__restrict__ gang, int4 *__restrict__ pre) {
     __shared__ int32_t sW[16];
     __shared__ int4 sCol[PLAN_MAX_COLS];
     __shared__ int32_t sK[PLAN_POD_CHUNK], sPcol[PLAN_POD_CHUNK];
+    __shared__ int32_t sGang[GANG ? PLAN_POD_CHUNK : 1];             // gang id of each staged pod (GANG only)
     __shared__ unsigned long long sRed[PLAN_WARPS];
     __shared__ unsigned long long sWin;
     __shared__ int32_t sF, sH[8];
@@ -198,110 +259,161 @@ plan_sequential(const int4 *__restrict__ topo4, int32_t *free_mask, const int4 *
     if (tid < 16) sW[tid] = W.w[tid];
     if (tid < ncol) sCol[tid] = __ldg(cols + tid);
     const int Ti = (int)T;
+    int64_t g_first = 0;                                              // GANG, block-uniform: first pod of the current gang,
+    int32_t g_id = 0;                                                 // its id (0: the pod is on its own)
+    bool g_failed = false;                                            // and whether one of its members has missed
     for (int64_t p0 = 0; p0 < P; p0 += PLAN_POD_CHUNK) {
         const int pn = (int)min((int64_t)PLAN_POD_CHUNK, P - p0);
         __syncthreads();
         for (int i = tid; i < pn; i += PLAN_THREADS) {
             sK[i] = __ldg(pods4 + p0 + i).x;
             sPcol[i] = __ldg(pcol + p0 + i);
+            if constexpr (GANG) sGang[i] = __ldg(gang + p0 + i);
         }
         __syncthreads();
 #pragma unroll 1
         for (int pi = 0; pi < pn; pi++) {
             const int64_t p = p0 + pi;
             const int c = sPcol[pi];                          // block-uniform
+            if constexpr (GANG) {
+                const int32_t id = sGang[pi];
+                if (id == 0 || id != g_id) {                  // a pod on its own, or the first member of a gang
+                    g_first = p;
+                    g_id = id;
+                    g_failed = false;
+                } else if (g_failed) {                        // a later member of a gang that has failed: not tried
+                    if (tid == 0) {
+                        keys[p] = ~0ull;
+                        victims[p] = 0;
+                    }
+                    continue;
+                }
+            }
             if (c < 0) {
                 if (tid == 0) {
                     keys[p] = (sK[pi] == 0 && N > 0) ? (unsigned long long)node_id_base << 8 : ~0ull;
                     victims[p] = 0;
                 }
-                continue;
-            }
-            // 1. the winner: the minimum over the tile minima of the pod's column
-            unsigned long long b = ~0ull;
-            for (int t = tid; t < Ti; t += PLAN_THREADS) b = min(b, tilekey[(int64_t)c * T + t]);
-            b = warp_min_u64_redux(b);
-            if (lane == 0) sRed[warp] = b;
-            __syncthreads();
-            if (warp == 0) {
-                b = warp_min_u64_redux(lane < PLAN_WARPS ? sRed[lane] : ~0ull);
-                if (lane == 0) {
-                    sWin = b;
-                    sNresc = 0;
-                    if (b == ~0ull) {
-                        keys[p] = ~0ull;
-                        victims[p] = 0;
-                    } else {
-                        // 2. the update of (F, H): victims from the working table, their GPUs freed, S taken
-                        const int64_t n = (int64_t)((b >> 8) & 0x7FFFFFFFull);
-                        const uint32_t S = (uint32_t)b & 0xFFu, cost = (uint32_t)(b >> 39) & 0x1FFFFu;
-                        const uint32_t f = (uint32_t)free_mask[n] & 0xFFu;
-                        int32_t h[8];
-                        uint32_t vic = 0;
+                if (!GANG || g_id == 0 || sK[pi] == 0) continue;
+            } else {
+                // 1. the winner: the minimum over the tile minima of the pod's column
+                unsigned long long b = ~0ull;
+                for (int t = tid; t < Ti; t += PLAN_THREADS) b = min(b, tilekey[(int64_t)c * T + t]);
+                b = warp_min_u64_redux(b);
+                if (lane == 0) sRed[warp] = b;
+                __syncthreads();
+                if (warp == 0) {
+                    b = warp_min_u64_redux(lane < PLAN_WARPS ? sRed[lane] : ~0ull);
+                    if (lane == 0) {
+                        sWin = b;
+                        sNresc = 0;
+                        if (b == ~0ull) {
+                            keys[p] = ~0ull;
+                            victims[p] = 0;
+                        } else {
+                            // 2. the update of (F, H): victims from the working table, their GPUs freed, S taken
+                            const int64_t n = (int64_t)((b >> 8) & 0x7FFFFFFFull);
+                            const uint32_t S = (uint32_t)b & 0xFFu, cost = (uint32_t)(b >> 39) & 0x1FFFFu;
+                            const uint32_t f = (uint32_t)free_mask[n] & 0xFFu;
+                            int32_t h[8];
+                            uint32_t vic = 0;
 #pragma unroll
-                        for (int g = 0; g < 8; g++) {
-                            h[g] = hold[n * 8 + g];
-                            if (((S & ~f) >> g) & 1u) vic |= 1u << (h[g] & 7);
+                            for (int g = 0; g < 8; g++) {
+                                h[g] = hold[n * 8 + g];
+                                if (((S & ~f) >> g) & 1u) vic |= 1u << (h[g] & 7);
+                            }
+                            if constexpr (GANG) {
+                                if (g_id != 0) {              // the pre-image of (F[n], H[n]) an undo restores
+                                    uint32_t lo = 0, hi = 0;
+#pragma unroll
+                                    for (int g = 0; g < 4; g++) {
+                                        lo |= ((uint32_t)h[g] & 0xFFu) << (8 * g);
+                                        hi |= ((uint32_t)h[g + 4] & 0xFFu) << (8 * g);
+                                    }
+                                    pre[p] = make_int4((int32_t)f, (int32_t)lo, (int32_t)hi, 0);
+                                }
+                            }
+                            uint32_t R = 0;
+#pragma unroll
+                            for (int g = 0; g < 8; g++)
+                                if (!((f >> g) & 1u) && h[g] >= 0 && ((vic >> (h[g] & 7)) & 1u)) R |= 1u << g;
+                            const uint32_t nf = (f | R) & ~S;
+#pragma unroll
+                            for (int g = 0; g < 8; g++) {
+                                if (((S | R) >> g) & 1u) h[g] = -1;
+                                hold[n * 8 + g] = h[g];
+                                sH[g] = h[g];
+                            }
+                            free_mask[n] = (int32_t)nf;
+                            sF = (int32_t)nf;
+                            keys[p] = ((unsigned long long)cost << 40) | ((unsigned long long)(node_id_base + n) << 8) | S;
+                            victims[p] = vic;
                         }
-                        uint32_t R = 0;
-#pragma unroll
-                        for (int g = 0; g < 8; g++)
-                            if (!((f >> g) & 1u) && h[g] >= 0 && ((vic >> (h[g] & 7)) & 1u)) R |= 1u << g;
-                        const uint32_t nf = (f | R) & ~S;
-#pragma unroll
-                        for (int g = 0; g < 8; g++) {
-                            if (((S | R) >> g) & 1u) h[g] = -1;
-                            hold[n * 8 + g] = h[g];
-                            sH[g] = h[g];
-                        }
-                        free_mask[n] = (int32_t)nf;
-                        sF = (int32_t)nf;
-                        keys[p] = ((unsigned long long)cost << 40) | ((unsigned long long)(node_id_base + n) << 8) | S;
-                        victims[p] = vic;
                     }
                 }
+                __syncthreads();
+                const unsigned long long win = sWin;
+                if (win == ~0ull) {                           // nothing changes
+                    if (!GANG || g_id == 0) continue;
+                } else {
+                    plan_refresh((int64_t)((win >> 8) & 0x7FFFFFFFull), topo4, mem4, Npad, T, ncol, pc, nodekey, tilekey, sW, sCol,
+                                 sF, sH, sResc, sNresc);
+                    continue;
+                }
             }
-            __syncthreads();
-            const unsigned long long win = sWin;
-            if (win == ~0ull) continue;                       // nothing changes
-            const int64_t n = (int64_t)((win >> 8) & 0x7FFFFFFFull);
-            const int64_t tile = n / PLAN_TILE;
-            // 3. every column's key of the winner's node under the new state; the tile minimum follows at once where it
-            //    can (the key went down, or the node did not hold the minimum), otherwise it is rescanned below
-            if (tid < ncol) {
-                PairCosts C;
-                plan_pair_costs(topo4, n, true, sW, C);
-                const uint32_t F = (uint32_t)sF & 0xFFu;
-                int32_t mem[8], h[8];
-                const int4 m0 = __ldg(mem4 + n * 2), m1 = __ldg(mem4 + n * 2 + 1);
-                mem[0] = m0.x; mem[1] = m0.y; mem[2] = m0.z; mem[3] = m0.w;
-                mem[4] = m1.x; mem[5] = m1.y; mem[6] = m1.z; mem[7] = m1.w;
+            if constexpr (GANG) {
+                // A member has missed: the members placed before it are undone, last first (k == 0 members took nothing).
+                __syncthreads();                              // once every thread is past this pod's reads of sF, sH
+                int64_t back = p;
+                unsigned long long key;
+#pragma unroll 1
+                while (--back >= g_first) {
+                    if (((key = keys[back]) & 0xFFull) == 0) continue;
+                    const int64_t n = (int64_t)((key >> 8) & 0xFFFFFFFFull) - node_id_base;
+                    if (tid == 0) {
+                        const int4 q = pre[back];
+                        free_mask[n] = q.x;
+                        sF = q.x;
 #pragma unroll
-                for (int g = 0; g < 8; g++) h[g] = sH[g];
-                uint64_t gm;
-                uint32_t lvp;
-                plan_owners(h, F, gm, lvp);
-                const unsigned long long old = tilekey[(int64_t)tid * T + tile];
-                const unsigned long long key = plan_node_key(C, pc, F, gm, lvp, mem, sCol[tid], n);
-                nodekey[(int64_t)tid * Npad + n] = key;
-                if (key < old) tilekey[(int64_t)tid * T + tile] = key;
-                else if (key != old && old != ~0ull && (int64_t)((old >> 8) & 0x7FFFFFFFull) == n) sResc[atomicAdd(&sNresc, 1)] = tid;
+                        for (int g = 0; g < 8; g++) {
+                            const int32_t v = (int32_t)(int8_t)(((uint32_t)(g < 4 ? q.y : q.z) >> (8 * (g & 3))) & 0xFFu);
+                            hold[n * 8 + g] = v;
+                            sH[g] = v;
+                        }
+                        sNresc = 0;
+                    }
+                    __syncthreads();
+                    plan_refresh(n, topo4, mem4, Npad, T, ncol, pc, nodekey, tilekey, sW, sCol, sF, sH, sResc, sNresc);
+                }
+                __syncthreads();                              // once every thread has read the keys
+                for (int64_t m = g_first + tid; m <= p; m += PLAN_THREADS) {     // every member gets NO_FIT and victims 0
+                    keys[m] = ~0ull;
+                    victims[m] = 0;
+                }
+                g_failed = true;
             }
-            __syncthreads();
-            // 4. rescans: warp per column, the 128 node keys of the tile
-            const int nr = sNresc;
-            for (int j = warp; j < nr; j += PLAN_WARPS) {
-                const int cc = sResc[j];
-                const unsigned long long *row = nodekey + (int64_t)cc * Npad + tile * PLAN_TILE;
-                unsigned long long m = ~0ull;
-#pragma unroll
-                for (int q = 0; q < PLAN_TILE / 32; q++) m = min(m, row[lane + 32 * q]);
-                m = warp_min_u64_redux(m);
-                if (lane == 0) tilekey[(int64_t)cc * T + tile] = m;
-            }
-            __syncthreads();
         }
     }
+}
+
+__global__ void __launch_bounds__(PLAN_THREADS, 1)
+plan_sequential(const int4 *__restrict__ topo4, int32_t *free_mask, const int4 *__restrict__ mem4, int32_t *hold, int64_t N,
+                int64_t Npad, int64_t T, int64_t node_id_base, const int4 *__restrict__ pods4, const int32_t *__restrict__ pcol,
+                int64_t P, const int4 *__restrict__ cols, int ncol, Weights W, PipeConsts pc, unsigned long long *nodekey,
+                unsigned long long *tilekey, unsigned long long *__restrict__ keys, uint32_t *__restrict__ victims) {
+    plan_sequential_body<false>(topo4, free_mask, mem4, hold, N, Npad, T, node_id_base, pods4, pcol, P, cols, ncol, W, pc, nodekey,
+                                tilekey, keys, victims, nullptr, nullptr);
+}
+
+// plan_sequential with gangs: gang[P] ids, pre[P] the members' pre-images (scratch).
+__global__ void __launch_bounds__(PLAN_THREADS, 1)
+gang_plan_sequential(const int4 *__restrict__ topo4, int32_t *free_mask, const int4 *__restrict__ mem4, int32_t *hold, int64_t N,
+                     int64_t Npad, int64_t T, int64_t node_id_base, const int4 *__restrict__ pods4, const int32_t *__restrict__ pcol,
+                     int64_t P, const int4 *__restrict__ cols, int ncol, Weights W, PipeConsts pc, unsigned long long *nodekey,
+                     unsigned long long *tilekey, unsigned long long *__restrict__ keys, uint32_t *__restrict__ victims,
+                     const int32_t *__restrict__ gang, int4 *__restrict__ pre) {
+    plan_sequential_body<true>(topo4, free_mask, mem4, hold, N, Npad, T, node_id_base, pods4, pcol, P, cols, ncol, W, pc, nodekey,
+                               tilekey, keys, victims, gang, pre);
 }
 
 }  // namespace kgpu

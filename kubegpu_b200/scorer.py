@@ -198,18 +198,28 @@ class Scorer:
                                                victims.ctypes.data))
         return keys, victims
 
-    def preempt_plan(self, pods, lvl):
+    def preempt_plan(self, pods, lvl, gang=None):
         """(keys uint64[P], victims uint32[P]) as preempt_batch, but conflict-free: pods are taken in order, each on the
         state the pods before it leave (their GPUs taken, their victims' GPUs free, neither evictable again).  Victim
-        sets are disjoint.  Dry run: the handle's masks and holder table are untouched.  Pass pods in priority order."""
+        sets are disjoint.  Dry run: the handle's masks and holder table are untouched.  Pass pods in priority order.
+        gang: int32[P] gang ids as for place_batch.  A gang's members evict and take all together or not at all: if a
+        member misses, the members before it are undone (their victims are running pods again for later pods) and the
+        whole gang gets NO_FIT and victims 0.  An id in two separate runs raises KgpuError (ERR_INVALID)."""
         pods, lvl = _i32(pods), _i32(lvl)
         P = pods.size // 4
         if lvl.size != P:
             raise ValueError("lvl must hold one level per pod")
         keys = np.empty(P, dtype=np.uint64)
         victims = np.empty(P, dtype=np.uint32)
-        self._check(self._L.kgpu_preempt_plan(self._h, pods.ctypes.data, lvl.ctypes.data, P, keys.ctypes.data,
-                                              victims.ctypes.data))
+        if gang is None:
+            self._check(self._L.kgpu_preempt_plan(self._h, pods.ctypes.data, lvl.ctypes.data, P, keys.ctypes.data,
+                                                  victims.ctypes.data))
+            return keys, victims
+        gang = _i32(gang)
+        if gang.size != P:
+            raise ValueError("gang must hold one id per pod")
+        self._check(self._L.kgpu_preempt_plan_gang(self._h, pods.ctypes.data, lvl.ctypes.data, gang.ctypes.data, P,
+                                                   keys.ctypes.data, victims.ctypes.data))
         return keys, victims
 
     def get_free_masks(self) -> np.ndarray:

@@ -188,6 +188,36 @@ def gen_preempt(N: int = 100_000, P: int = 10_000, seed: int = SEED_PREEMPT):
     return topo, free, hold, pods, lvl
 
 
+SEED_PREEMPT_GANGS = 0xB2000009
+
+
+def gen_preempt_gangs(N: int = 20_000, P: int = 10_000, seed: int = SEED_PREEMPT_GANGS, gang_start: float = 0.1):
+    """gen_preempt's almost full cluster and pods, with high-priority training jobs mixed in: at each pod that is not yet
+    in a gang, a gang starts with probability ``gang_start`` (about a third of the pods end up in gangs).  A gang has
+    2..8 consecutive members, one level in 1..4, and each member's k is drawn from {4, 8} on its own.  Mixed k within a
+    gang is what makes a member miss after earlier members were given victims; the default 20k nodes keep the cluster
+    small enough that such gangs occur (at 100k nodes none fails).  Ids are 1, 2, ... in order.
+    Returns (topo, free, holders[N][8], pods, lvl[P], gang[P])."""
+    topo, free, hold, pods, lvl = gen_preempt(N, P, seed)
+    start = rand_below(seed, 61, P, 1 << 20) < int(gang_start * (1 << 20))
+    size = 2 + rand_below(seed, 62, P, 7)
+    glvl = (1 + rand_below(seed, 63, P, 4)).astype(np.int32)
+    kg = np.array([4, 8], dtype=np.int32)[rand_below(seed, 64, P, 2)]
+    gang = np.zeros(P, dtype=np.int32)
+    p, gid = 0, 0
+    while p < P:
+        if start[p]:
+            gid += 1
+            end = min(P, p + int(size[p]))
+            gang[p:end] = gid
+            lvl[p:end] = glvl[p]
+            pods[p:end, 0] = kg[p:end]
+            p = end
+        else:
+            p += 1
+    return topo, free, hold, pods, lvl, gang
+
+
 def gen_gangs(N: int = 100_000, P: int = 10_000, seed: int = SEED_GANGS, gang_start: float = 0.1):
     """C2's cluster and pod stream, with distributed training jobs mixed in: at each pod that is not yet in a gang,
     a gang starts with probability ``gang_start`` (default: about a third of the pods end up in gangs).  A gang has
