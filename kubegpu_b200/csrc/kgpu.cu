@@ -94,6 +94,8 @@ struct kgpu_shard {
     std::vector<kgpu::SparseWorkItem> h_work;   // K1s work list for work_P pods (sparse_work.h)
     kgpu::DeviceBuffer<int4> d_work;
     int64_t work_P = -1;
+    bool work_aligned = false;                  // its pod ranges are whole chunks: K1s launches take prepared chunk tables
+    kgpu::DeviceBuffer<int4> d_chunks;          // [chunks][SP_CHUNK_INT4] sp_prepare_chunks: the batch's sorted pod tables
     bool tma_attr_done = false;                 // cudaFuncSetAttribute of the TMA instantiations done on this device
     kgpu::DeviceBuffer<uint32_t> d_nodebest;    // [views][9][Npad]  K3 tables
     kgpu::DeviceBuffer<int32_t> d_half;         // [Npad][96]  K3: half tables of every node (place_half_tables)
@@ -410,6 +412,7 @@ int launch_score(kgpu_ctx *h, kgpu_shard &s, const int32_t *d_pods, int64_t P, u
                                              : P <= kgpu::kSparseChunk               ? (int64_t)s.sm_count * KGPU_SP_STREAM_MINBLOCKS
                                                                                      : resident;
                     kgpu::build_sparse_work(s.tile_class, P, res_list, s.h_work, prm);
+                    s.work_aligned = kgpu::sparse_work_chunk_aligned((int64_t)s.tile_class.size(), P, res_list, prm);
                     KGPU_CUDA(h, s.d_work.reserve((int64_t)s.h_work.size()));
                     static_assert(sizeof(kgpu::SparseWorkItem) == sizeof(int4), "work item layout");
                     KGPU_CUDA(h, cudaMemcpyAsync(s.d_work, s.h_work.data(), s.h_work.size() * sizeof(int4), cudaMemcpyHostToDevice, st));
@@ -418,11 +421,26 @@ int launch_score(kgpu_ctx *h, kgpu_shard &s, const int32_t *d_pods, int64_t P, u
                 d_work = s.d_work;
                 grid = dim3((unsigned)s.h_work.size(), 1);
             }
+            // Whole-chunk pod ranges: every chunk's pod table is built once for the launch (sp_prepare_chunks, on the
+            // same stream just before each K1s launch) rather than by each of the ~900 blocks that score it (C2).
+            const bool prepared = use_work && s.work_aligned;
+            const int64_t n_chunks = (P + kgpu::SP_CHUNK - 1) / kgpu::SP_CHUNK;
+            if (prepared) {
+                if (n_chunks > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "batch too large for one launch");
+                const int64_t cap_chunks = (pod_headroom(P) + kgpu::SP_CHUNK - 1) / kgpu::SP_CHUNK;
+                KGPU_CUDA(h, s.d_chunks.reserve(n_chunks * kgpu::SP_CHUNK_INT4, cap_chunks * kgpu::SP_CHUNK_INT4));
+            }
+            const int4 *d_chunks = prepared ? s.d_chunks.get() : nullptr;
+#define KGPU_PREPARE_CHUNKS(MEMF)                                                                             \
+    if (prepared) {                                                                                           \
+        kgpu::sp_prepare_chunks<MEMF><<<(unsigned)n_chunks, kgpu::SP_THREADS, 0, st>>>(pods4, P, s.d_flag, s.d_chunks); \
+        h->launches++;                                                                                        \
+    }
             bool byte_keys = true;       // every cost < 2^16 <=> 28 * max weight < 65536
             for (int i = 0; i < 16; i++) byte_keys = byte_keys && h->W[i] <= 2340;
 #define KGPU_LAUNCH_SPARSE(MEMF, BK, ST)                                                                      \
     kgpu::score_pairs_sparse<true, MEMF, BK, ST><<<grid, kgpu::SP_THREADS, 0, st>>>(                          \
-        s.d_rec, s.d_meta, s.d_mem, s.d_order, s.d_flag, s.node_id_base, pods4, P, (int)per, d_work, PC, d_keys)
+        s.d_rec, s.d_meta, s.d_mem, s.d_order, s.d_flag, s.node_id_base, pods4, P, (int)per, d_work, PC, d_keys, d_chunks)
 #define KGPU_LAUNCH_SPARSE_TMA(BK, MB)                                                                        \
     kgpu::score_pairs_sparse<true, false, BK, true, MB><<<grid, kgpu::SP_THREADS, kgpu::SP_TMA_DYN_SMEM, st>>>(   \
         s.d_rec, s.d_meta, s.d_mem, s.d_order, s.d_flag, s.node_id_base, pods4, P, (int)per, d_work, PC, d_keys)
@@ -441,13 +459,18 @@ int launch_score(kgpu_ctx *h, kgpu_shard &s, const int32_t *d_pods, int64_t P, u
             if (sparse_main) {
                 if (tma_build) { if (byte_keys) KGPU_LAUNCH_SPARSE_TMA(true, KGPU_SP_TMA_MINBLOCKS); else KGPU_LAUNCH_SPARSE_TMA(false, KGPU_SP_TMA_MINBLOCKS); }
                 else if (stream_build) { if (byte_keys) KGPU_LAUNCH_SPARSE(false, true, true); else KGPU_LAUNCH_SPARSE(false, false, true); }
-                else                   { if (byte_keys) KGPU_LAUNCH_SPARSE(false, true, false); else KGPU_LAUNCH_SPARSE(false, false, false); }
+                else {
+                    KGPU_PREPARE_CHUNKS(false)
+                    if (byte_keys) KGPU_LAUNCH_SPARSE(false, true, false); else KGPU_LAUNCH_SPARSE(false, false, false);
+                }
                 h->launches++;
             }
             if (has_mem != 0) {
+                KGPU_PREPARE_CHUNKS(true)
                 if (byte_keys) KGPU_LAUNCH_SPARSE(true, true, false); else KGPU_LAUNCH_SPARSE(true, false, false);
                 h->launches++;
             }
+#undef KGPU_PREPARE_CHUNKS
 #undef KGPU_LAUNCH_SPARSE
 #undef KGPU_LAUNCH_SPARSE_TMA
         } else if (has_mem != 0) {   // K1m: the memory-constrained pods (its blocks exit at once if the flag is 0)

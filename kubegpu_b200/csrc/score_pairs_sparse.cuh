@@ -73,12 +73,116 @@ constexpr int SP_MEM_SUB = 4;        // MEM launch: pods of one k are sub-bucket
 // positions of a chunk of CH pods (nine padded buckets, then the pods not for this launch), rounded to whole
 // trips, plus one trip: the prefetch build reads one past a bucket's end
 __host__ __device__ constexpr int sp_tab_len(int CH) { return (CH + 9 * (SP_PAD - 1) + SP_PAD - 1) / SP_PAD * SP_PAD + SP_PAD; }
+// What the pod sort makes of a chunk.  It depends on the chunk's pods only, never on the tile, so for a launch over
+// many pods sp_prepare_chunks builds it once per chunk into global memory in exactly this layout, and a block copies
+// it in with 16-byte loads instead of sorting.
+template <int N>
+struct alignas(16) SpChunkTab {
+    uint32_t one[N];                 // MEM: the pods' min_mem instead (the MEM loops derive `one` from K)
+    uint16_t idx[N];                 // bucket-order position -> chunk position (SP_DUMMY: padding)
+    int32_t off[12];                 // off[k]: where bucket k starts; off[9]: end of the served pods; off[11]: bit k = bucket k has pods
+};
 template <int N>
 struct alignas(16) SpTab {
-    uint32_t one[N];                 // MEM: the pods' min_mem instead (the MEM loops derive `one` from K)
+    SpChunkTab<N> c;
     uint32_t best[SP_WARPS][N];      // warp key of the best (node, subset) of this warp for the pod, INF32 = none
 };
 static_assert(sp_tab_len(SP_CHUNK) % 4 == 0, "rows of the pod table must stay 16-byte aligned");
+constexpr int SP_POS = sp_tab_len(SP_CHUNK);
+constexpr int SP_CHUNK_INT4 = (int)(sizeof(SpChunkTab<SP_POS>) / 16);      // 16-byte words of a prepared chunk table: 207
+static_assert(sizeof(SpChunkTab<SP_POS>) % 16 == 0, "prepared chunk tables are copied in 16-byte words");
+
+// The chunk's pod sort: pods4[0..cn), cn <= CH, into `tab` in bucket order -- the pods that want k GPUs for k = 0..8
+// (MEM: sub-bucketed by a hash of min_mem), each k padded with dummy pods to a multiple of SP_PAD, then the pods not for
+// this launch (k outside 0..8, or on the other side of min_mem).  cnt: NB shared counters.  acc != nullptr: the
+// positions' running minima of a multi-tile item are reset as well.  All NT threads of the block call it, between two
+// barriers of the caller's (the table is only read after the second).
+template <bool MEM, int CH, int NT, int N>
+__device__ __forceinline__ void sp_sort_chunk(const int4 *__restrict__ pods4, int cn, int32_t *cnt, SpChunkTab<N> &tab,
+                                              unsigned long long *acc, int tid) {
+    constexpr int SUB = MEM ? SP_MEM_SUB : 1, NB = 9 * SUB + 1;
+    constexpr int PPT = (CH + NT - 1) / NT;            // pods per thread
+    if (tid < NB) cnt[tid] = 0;
+    __syncthreads();
+    // each thread keeps its pods' buckets and multipliers in registers from the count to the scatter
+    int bkt[PPT];
+    uint32_t mult[PPT];
+#pragma unroll
+    for (int u = 0; u < PPT; u++) {
+        const int i = tid + u * NT;
+        bkt[u] = 9 * SUB;
+        mult[u] = 0;
+        if (i < cn) {
+            const int4 req = __ldg(pods4 + i);
+            const bool wants_mem = req.w > 0;
+            if (req.x >= 0 && req.x <= 8 && wants_mem == MEM)
+                bkt[u] = req.x * SUB + (MEM ? (int)(((uint32_t)req.w * 0x9E3779B1u) >> 30) : 0);
+            // the per-pod multiplier: the pod's own k less what its bucket adds back (= 1 at run time)
+            mult[u] = MEM ? (uint32_t)req.w : (uint32_t)(req.x - (bkt[u] < 9 ? bkt[u] - 1 : 0));
+            atomicAdd(&cnt[bkt[u]], 1);
+        }
+    }
+    __syncthreads();
+    if (tid < 32) {                                    // warp 0, lane k: bucket k.  off[k]: where k's pods start; cnt: running positions
+        const int k = tid;
+        int c_sub[SUB], c = 0;
+#pragma unroll
+        for (int u = 0; u < SUB; u++) { c_sub[u] = k < 9 ? cnt[k * SUB + u] : 0; c += c_sub[u]; }
+        const int padded = (c + SP_PAD - 1) / SP_PAD * SP_PAD;
+        int end = padded;                              // inclusive prefix sum over lanes 0..8
+#pragma unroll
+        for (int d = 1; d < 16; d <<= 1) {
+            const int t = __shfl_up_sync(0xFFFFFFFFu, end, d);
+            if (k >= d) end += t;
+        }
+        const int served = __shfl_sync(0xFFFFFFFFu, end, 8);
+        const uint32_t nonempty = __ballot_sync(0xFFFFFFFFu, c > 0);
+        if (k < 9) {
+            int a = end - padded;
+            tab.off[k] = a;
+#pragma unroll
+            for (int u = 0; u < SUB; u++) { cnt[k * SUB + u] = a; a += c_sub[u]; }
+            for (; a < end; a++) {                     // dummy pods up to the next multiple of SP_PAD
+                tab.idx[a] = SP_DUMMY;
+                tab.one[a] = MEM ? 0u : 1u;
+            }
+        } else if (k == 9) {
+            cnt[9 * SUB] = served;                     // the pods not for this launch follow bucket 8
+            tab.off[9] = served;
+            tab.off[10] = 0;
+            tab.off[11] = (int)nonempty;
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int u = 0; u < PPT; u++) {
+        const int i = tid + u * NT;
+        if (i < cn) {
+            const int at = atomicAdd(&cnt[bkt[u]], 1);
+            tab.idx[at] = (uint16_t)i;
+            if (acc) acc[at] = ~0ull;
+            tab.one[at] = mult[u];
+        }
+    }
+}
+
+// One block per SP_CHUNK pods of the batch: the chunk's sorted pod table (sp_sort_chunk, as a K1s block would make it)
+// into chunks[chunk][SP_CHUNK_INT4].  Launched before a K1s launch over more than one chunk of pods, on its stream;
+// the K1s blocks whose pod range covers a whole chunk (or ends at P) copy the table instead of sorting.
+template <bool MEM>
+__global__ void __launch_bounds__(SP_THREADS)
+sp_prepare_chunks(const int4 *__restrict__ pods4, int64_t P, const int *__restrict__ mem_flag, int4 *__restrict__ chunks) {
+    if (MEM && *mem_flag == 0) return;                 // (the MEM K1s launch exits at once as well)
+    constexpr int NB = 9 * (MEM ? SP_MEM_SUB : 1) + 1;
+    __shared__ int32_t sCnt[NB];
+    __shared__ SpChunkTab<SP_POS> sChunk;
+    const int tid = threadIdx.x;
+    const int64_t c0 = (int64_t)blockIdx.x * SP_CHUNK;
+    sp_sort_chunk<MEM, SP_CHUNK, SP_THREADS>(pods4 + c0, (int)min((int64_t)SP_CHUNK, P - c0), sCnt, sChunk, nullptr, tid);
+    __syncthreads();
+    int4 *const dst = chunks + (int64_t)blockIdx.x * SP_CHUNK_INT4;
+    for (int q = tid; q < SP_CHUNK_INT4; q += SP_THREADS) dst[q] = reinterpret_cast<const int4 *>(&sChunk)[q];
+}
 
 // Pods per trip of the (K, F) bucket loop.  Four share the multiplier load, the result store and the loop
 // control; two where four pods' enumerations in flight push values into local memory (cuobjdump -sass).  The
@@ -393,16 +497,18 @@ __global__ void __launch_bounds__(SP_THREADS, TMA ? TMA : STREAM ? KGPU_SP_STREA
 score_pairs_sparse(const int4 *__restrict__ rec, const uint32_t *__restrict__ meta,
                    const int32_t *__restrict__ gpu_mem, const int32_t *__restrict__ order,
                    const int *__restrict__ mem_flag, int64_t node_id_base, const int4 *__restrict__ pods4, int64_t P,
-                   int pods_per_split, const int4 *__restrict__ work, PipeConsts pc, unsigned long long *__restrict__ keys) {
+                   int pods_per_split, const int4 *__restrict__ work, PipeConsts pc, unsigned long long *__restrict__ keys,
+                   const int4 *__restrict__ chunks = nullptr /*sp_prepare_chunks' tables of this batch, or none*/) {
     if (MEM && *mem_flag == 0) return;
     static_assert(!TMA || (STREAM && !MEM), "the TMA instantiation is a streaming one");
     constexpr int SUB = MEM ? SP_MEM_SUB : 1, NB = 9 * SUB + 1;     // sort buckets: (k, sub) for k = 0..8, then "not for this launch"
     constexpr int CH = TMA ? SP_TMA_PODS : SP_CHUNK;                // pods per chunk of the block's pod sort
     constexpr int POS = sp_tab_len(CH);                // bucket-order positions
-    constexpr int PPT = (CH + SP_THREADS - 1) / SP_THREADS;         // pods per thread in the pod sort
-    __shared__ int32_t sCnt[NB], sOff[12];             // sOff[11]: bit k set = bucket k has pods (STREAM builds test it per tile)
-    __shared__ uint16_t sIdx[POS];                     // bucket-order position -> chunk position (SP_DUMMY: padding)
-    __shared__ SpTab<POS> sTab;                        // bucket order: multipliers | per-warp results
+    __shared__ int32_t sCnt[NB];
+    __shared__ SpTab<POS> sTab;                        // bucket order: multipliers, positions, offsets | per-warp results
+    __shared__ int32_t sF[SP_WARPS];                   // !STREAM: every warp's F, so that a block skips the k no slot can serve
+    uint16_t (&sIdx)[POS] = sTab.c.idx;
+    int32_t (&sOff)[12] = sTab.c.off;                  // sOff[11]: bit k set = bucket k has pods (STREAM builds test it per tile)
     // position g -> byte (1 << GPU index), g = 0..3 | 4..7.  STREAM builds (few pods per tile) keep the slot's
     // permutation word in sHotLo instead and expand the winner's S' in the flush: per pod, not per node.
     __shared__ uint32_t sHotLo[SP_THREADS], sHotHi[STREAM ? 1 : SP_THREADS];
@@ -543,80 +649,35 @@ score_pairs_sparse(const int4 *__restrict__ rec, const uint32_t *__restrict__ me
         for (int g = 0; g < 8; g++) mem[g] = __ldg(gpu_mem + (int64_t)node * 8 + ((pm >> (3 * g)) & 7u));
     }
     const int F = (int)__reduce_max_sync(0xFFFFFFFFu, nfree);    // warp-uniform bound on usable positions
+    if (!STREAM && lane_field == 0) sF[tid >> 5] = F;             // read after the first chunk's prologue barrier
 
     for (int64_t c0 = p_begin; c0 < p_end; c0 += CH) {
         const int cn = (int)min((int64_t)CH, p_end - c0);
-        if (!multi || tt == 0) {                   // the chunk's pod sort (once per item when it walks several tiles)
+        if (!multi || tt == 0) {                   // the chunk's pod table (once per item when it walks several tiles)
         __syncthreads();
-        if (tid < NB) sCnt[tid] = 0;
-        __syncthreads();
-        // each thread keeps its pods' buckets and multipliers in registers from the count to the scatter
-        int bkt[PPT];
-        uint32_t mult[PPT];
-#pragma unroll
-        for (int u = 0; u < PPT; u++) {
-            const int i = tid + u * SP_THREADS;
-            bkt[u] = 9 * SUB;
-            mult[u] = 0;
-            if (i < cn) {
-                const int4 req = __ldg(pods4 + c0 + i);
-                const bool wants_mem = req.w > 0;
-                if (req.x >= 0 && req.x <= 8 && wants_mem == MEM)
-                    bkt[u] = req.x * SUB + (MEM ? (int)(((uint32_t)req.w * 0x9E3779B1u) >> 30) : 0);
-                // the per-pod multiplier: the pod's own k less what its bucket adds back (= 1 at run time)
-                mult[u] = MEM ? (uint32_t)req.w : (uint32_t)(req.x - (bkt[u] < 9 ? bkt[u] - 1 : 0));
-                atomicAdd(&sCnt[bkt[u]], 1);
-            }
+        // a whole chunk of the batch (or its last, up to P): its table was prepared for the launch -- one coalesced copy
+        if (!STREAM && !multi && chunks != nullptr && c0 % CH == 0 && (c0 + CH <= p_end || p_end == P)) {
+            const int4 *const src = chunks + (c0 / CH) * SP_CHUNK_INT4;
+            for (int q = tid; q < SP_CHUNK_INT4; q += SP_THREADS) reinterpret_cast<int4 *>(&sTab.c)[q] = __ldg(src + q);
+        } else {
+            sp_sort_chunk<MEM, CH, SP_THREADS>(pods4 + c0, cn, sCnt, sTab.c, CAN_MULTI && multi ? sAcc : nullptr, tid);
         }
         __syncthreads();
-        if (tid < 32) {                            // warp 0, lane k: bucket k.  sOff[k]: where k's pods start; sCnt: running positions
-            const int k = tid;
-            int cnt[SUB], c = 0;
-#pragma unroll
-            for (int u = 0; u < SUB; u++) { cnt[u] = k < 9 ? sCnt[k * SUB + u] : 0; c += cnt[u]; }
-            const int padded = (c + SP_PAD - 1) / SP_PAD * SP_PAD;
-            int end = padded;                      // inclusive prefix sum over lanes 0..8
-#pragma unroll
-            for (int d = 1; d < 16; d <<= 1) {
-                const int t = __shfl_up_sync(0xFFFFFFFFu, end, d);
-                if (k >= d) end += t;
-            }
-            const int served = __shfl_sync(0xFFFFFFFFu, end, 8);
-            const uint32_t nonempty = __ballot_sync(0xFFFFFFFFu, c > 0);
-            if (k < 9) {
-                int acc = end - padded;
-                sOff[k] = acc;
-#pragma unroll
-                for (int u = 0; u < SUB; u++) { sCnt[k * SUB + u] = acc; acc += cnt[u]; }
-                for (; acc < end; acc++) {         // dummy pods up to the next multiple of SP_PAD
-                    sIdx[acc] = SP_DUMMY;
-                    sTab.one[acc] = MEM ? 0u : 1u;
-                }
-            } else if (k == 9) {
-                sCnt[9 * SUB] = served;            // the pods not for this launch follow bucket 8
-                sOff[9] = served;
-                sOff[11] = (int)nonempty;
-            }
-        }
-        __syncthreads();
-#pragma unroll
-        for (int u = 0; u < PPT; u++) {
-            const int i = tid + u * SP_THREADS;
-            if (i < cn) {
-                const int at = atomicAdd(&sCnt[bkt[u]], 1);
-                sIdx[at] = (uint16_t)i;
-                if (multi) sAcc[at] = ~0ull;
-                sTab.one[at] = mult[u];
-            }
-        }
-        __syncthreads();
-        }   // pod sort
+        }   // pod table
 
         // few pods per tile: most buckets are empty and nine (two loads, compare, branch) prologues per tile show; one
         // word says which buckets to enter
         const uint32_t kmask = STREAM ? (uint32_t)sOff[11] : 0x1FFu;
+        // k above every warp's F: no slot of the tile can serve those pods, so their buckets are neither entered (no
+        // rows of INF32) nor flushed.  (A multi-tile item reads its chunk's table once, before the barrier sF needs.)
+        int fb = 8;
+        if (!STREAM && !multi) {
+            fb = sF[0];
+#pragma unroll
+            for (int w = 1; w < SP_WARPS; w++) fb = max(fb, (int)sF[w]);
+        }
 #define KGPU_SP_RUN(K) \
-        if (!STREAM || ((kmask >> K) & 1u)) sp_run_k<K, PER_PAIR, MEM, BYTE_KEYS>(F, C, pc, nfree, valid, mem, lane_field, sTab.one, best_row, sOff[K], sOff[K + 1]);
+        if ((!STREAM || ((kmask >> K) & 1u)) && K <= fb) sp_run_k<K, PER_PAIR, MEM, BYTE_KEYS>(F, C, pc, nfree, valid, mem, lane_field, sTab.c.one, best_row, sOff[K], sOff[K + 1]);
         KGPU_SP_RUN(0) KGPU_SP_RUN(1) KGPU_SP_RUN(2) KGPU_SP_RUN(3) KGPU_SP_RUN(4) KGPU_SP_RUN(5) KGPU_SP_RUN(6) KGPU_SP_RUN(7) KGPU_SP_RUN(8)
 #undef KGPU_SP_RUN
         __syncthreads();
@@ -625,7 +686,7 @@ score_pairs_sparse(const int4 *__restrict__ rec, const uint32_t *__restrict__ me
         // winner's one-hot bytes, REDG.MIN.64 into keys[pod].  Ordered tile + byte keys: the warp index goes
         // into bits 13.. of the warp key (its lane byte has 3 spare bits) and plain 32-bit mins decide;
         // otherwise (a tile of two classes) node ids are compared explicitly.
-        const int served = sOff[9];                // bucket 9 (not for this launch) sits at the end
+        const int served = sOff[min(fb, 8) + 1];   // the buckets above fb, then bucket 9 (not for this launch), sit at the end
         for (int i = tid; i < served; i += SP_THREADS) {
             if (sIdx[i] == SP_DUMMY) continue;
             uint32_t best_m = INF32, cost = 0;

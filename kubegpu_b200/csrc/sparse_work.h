@@ -8,7 +8,8 @@
 // by two orders of magnitude (a long tail at the end of the launch), and with few tiles (a
 // shard of a multi-GPU run) either too few blocks or ranges so short that staging and the per-chunk pod sort
 // dominate.  The work list cuts the (tile, pod) plane into items of about equal WORK instead, heaviest first:
-//   * many pods:  an item is one tile x a pod range (several chunks of the block's pod sort);
+//   * many pods:  an item is one tile x a pod range (several chunks of the block's pod sort); on planes with enough
+//     (tile, chunk) cells the ranges are whole chunks, whose sorted pod tables are built once per launch;
 //   * few pods (the whole batch fits one chunk -- the HBM-bound regime, where the node records are streamed
 //     once and hardly reused): an item is a RUN of consecutive tiles x all pods; the block sorts the pods once,
 //     keeps the per-pod running minimum in shared memory across its tiles and flushes it once.
@@ -41,8 +42,19 @@ struct SparseWorkParams {
                                 // 0.624 / 2.382 ms for 1, 0.425 / 1.636 for 4, 0.427 / 1.587 for 16, 0.478 / 1.637 for 64)
 };
 
+// Many pods: do the pod ranges start and end on whole chunks (or end at P)?  Then every block takes its chunks' pod
+// tables from the ones sp_prepare_chunks builds once per launch instead of sorting each chunk itself.  Only when the
+// plane has at least `waves` such (tile, chunk) cells per resident block: on a small shard (C5's 10k nodes: ~80 tiles
+// x 20 chunks) whole chunks leave too few items, and 32-pod ranges with the block's own sort are faster.
+inline bool sparse_work_chunk_aligned(int64_t tiles, int64_t P, int64_t resident_blocks,
+                                      const SparseWorkParams prm = SparseWorkParams()) {
+    if (P <= kSparseChunk) return false;
+    return tiles * ((P + kSparseChunk - 1) / kSparseChunk) >= std::max<int64_t>(1, prm.waves * resident_blocks);
+}
+
 // `out` = the items in launch order (heaviest first; the grid runs them in index order); `weight_out`, if
-// given, receives their model cost.  Pod ranges are multiples of 32 pods.
+// given, receives their model cost.  Pod ranges are multiples of 32 pods, and of kSparseChunk pods (or end at P)
+// when sparse_work_chunk_aligned says so.
 inline void build_sparse_work(const std::vector<uint8_t> &tile_class, int64_t P, int64_t resident_blocks,
                               std::vector<SparseWorkItem> &out, const SparseWorkParams prm = SparseWorkParams(),
                               std::vector<int64_t> *weight_out = nullptr) {
@@ -54,6 +66,7 @@ inline void build_sparse_work(const std::vector<uint8_t> &tile_class, int64_t P,
     int64_t total = 0;
     for (uint8_t f : tile_class) total += kSparseTileCost + P * kSparsePodCost[std::min<int>(f, 8)];
     const int64_t slots = std::max<int64_t>(1, prm.waves * resident_blocks);
+    const int64_t gran = sparse_work_chunk_aligned((int64_t)tile_class.size(), P, resident_blocks, prm) ? kSparseChunk : 32;
     if (P <= kSparseChunk) {
         // few pods: runs of consecutive tiles, cut when the run's work reaches the target
         const int64_t target = std::max<int64_t>(total / slots, 2 * kSparseFixedCost);
@@ -78,8 +91,8 @@ inline void build_sparse_work(const std::vector<uint8_t> &tile_class, int64_t P,
         const int64_t tail_percent = prm.tail_percent >= 0 ? prm.tail_percent : ((int64_t)tile_class.size() * 4 >= resident_blocks ? 15 : 0);
         for (size_t t = 0; t < tile_class.size(); t++) {
             const int64_t c = kSparsePodCost[std::min<int>(tile_class[t], 8)];
-            const int64_t per = std::max<int64_t>(32, (target - kSparseFixedCost) / c / 32 * 32);
-            const int64_t small = std::max<int64_t>(32, per / std::max<int64_t>(1, prm.tail_div) / 32 * 32);
+            const int64_t per = std::max<int64_t>(gran, (target - kSparseFixedCost) / c / gran * gran);
+            const int64_t small = std::max<int64_t>(gran, per / std::max<int64_t>(1, prm.tail_div) / gran * gran);
             const int64_t big_end = P * (100 - tail_percent) / 100 / per * per;
             int64_t b = 0;
             while (b < P) {
