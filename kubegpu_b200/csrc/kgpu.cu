@@ -26,6 +26,7 @@
 #include "score_pairs.cuh"
 #include "score_pairs_sparse.cuh"
 #include "node_state.cuh"
+#include "launch_plan.h"
 
 namespace {
 
@@ -97,6 +98,7 @@ struct kgpu_shard {
     bool work_aligned = false;                  // its pod ranges are whole chunks: K1s launches take prepared chunk tables
     kgpu::DeviceBuffer<int4> d_chunks;          // [chunks][SP_CHUNK_INT4] sp_prepare_chunks: the batch's sorted pod tables
     bool tma_attr_done = false;                 // cudaFuncSetAttribute of the TMA instantiations done on this device
+    bool place_attr_done = false;               // the same for place_sequential<false / true> (PLACE_DYN_SMEM)
     kgpu::DeviceBuffer<uint32_t> d_nodebest;    // [views][9][Npad]  K3 tables
     kgpu::DeviceBuffer<int32_t> d_half;         // [Npad][96]  K3: half tables of every node (place_half_tables)
     kgpu::DeviceBuffer<unsigned long long> d_tilebest;   // [views][9][T]
@@ -152,13 +154,7 @@ int fail(kgpu_ctx *h, int code, const char *fmt, ...) {
 int upload_subset_tables(kgpu_ctx *h) {
     uint8_t subs[9][70];
     uint8_t nsub[9];
-    memset(subs, 0, sizeof subs);
-    for (int k = 0; k <= 8; k++) {
-        int c = 0;
-        for (unsigned S = 0; S < 256; S++)
-            if (__builtin_popcount(S) == k) subs[k][c++] = (uint8_t)S;
-        nsub[k] = (uint8_t)c;
-    }
+    kgpu::subset_tables(subs, nsub);
     for (auto &s : h->shards) {
         KGPU_CUDA(h, cudaSetDevice(s.dev));
         KGPU_CUDA(h, cudaMemcpyToSymbol(kgpu::c_subsets, subs, sizeof subs));
@@ -213,16 +209,7 @@ int build_order(kgpu_ctx *h, kgpu_shard &s) {
     }
     for (int c = 0; c < 9; c++) s.class_count[c] = meta[c];
     s.n_slots = meta[9];
-    // max free count per tile, from the class layout: class c's nodes sit in [start, start + count)
-    s.tile_class.assign((size_t)(s.n_slots / kgpu::SP_THREADS), 0);
-    int64_t start = 0;
-    for (int c = 8; c >= 0; c--) {
-        const int64_t cnt = s.class_count[c];
-        if (cnt > 0)
-            for (int64_t t = start / kgpu::SP_THREADS; t <= (start + cnt - 1) / kgpu::SP_THREADS; t++)
-                s.tile_class[(size_t)t] = std::max<uint8_t>(s.tile_class[(size_t)t], (uint8_t)c);
-        start += (cnt + kOrderPad - 1) / kOrderPad * kOrderPad;
-    }
+    s.tile_class = kgpu::tile_classes(s.class_count, kOrderPad, s.n_slots);
     s.work_P = -1;
     s.order_dirty = false;
     s.stale_nodes = 0;
@@ -370,8 +357,7 @@ int launch_score(kgpu_ctx *h, kgpu_shard &s, const int32_t *d_pods, int64_t P, u
     int64_t splits = std::max<int64_t>(1, (waves * resident + tiles - 1) / tiles);
     splits = std::min<int64_t>(splits, std::max<int64_t>(1, P / 128));
     splits = std::min<int64_t>(splits, 65535);
-    int64_t per = (P + splits - 1) / splits;
-    per = (per + 31) / 32 * 32;
+    const int64_t per = kgpu::pods_per_split(P, splits);
     splits = (P + per - 1) / per;
     if (tiles > 0x7FFFFFFFLL || per > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "batch too large for one launch");
     dim3 grid((unsigned)tiles, (unsigned)splits);
@@ -408,9 +394,7 @@ int launch_score(kgpu_ctx *h, kgpu_shard &s, const int32_t *d_pods, int64_t P, u
                     if (env_tail >= 0) prm.tail_percent = env_tail;
                     if (env_waves > 0) prm.waves = env_waves;
                     if (env_floor > 0) prm.floor = env_floor;
-                    const int64_t res_list = (tma_mode != 0 && P <= kgpu::SP_TMA_PODS) ? (int64_t)s.sm_count * KGPU_SP_TMA_MINBLOCKS
-                                             : P <= kgpu::kSparseChunk               ? (int64_t)s.sm_count * KGPU_SP_STREAM_MINBLOCKS
-                                                                                     : resident;
+                    const int64_t res_list = kgpu::sparse_list_resident(P, tma_mode, s.sm_count, resident);
                     kgpu::build_sparse_work(s.tile_class, P, res_list, s.h_work, prm);
                     s.work_aligned = kgpu::sparse_work_chunk_aligned((int64_t)s.tile_class.size(), P, res_list, prm);
                     KGPU_CUDA(h, s.d_work.reserve((int64_t)s.h_work.size()));
@@ -423,56 +407,36 @@ int launch_score(kgpu_ctx *h, kgpu_shard &s, const int32_t *d_pods, int64_t P, u
             }
             // Whole-chunk pod ranges: every chunk's pod table is built once for the launch (sp_prepare_chunks, on the
             // same stream just before each K1s launch) rather than by each of the ~900 blocks that score it (C2).
-            const bool prepared = use_work && s.work_aligned;
+            const kgpu::SparseRoute route = kgpu::sparse_route(P, use_work, s.work_aligned, tma_mode, h->W);
             const int64_t n_chunks = (P + kgpu::SP_CHUNK - 1) / kgpu::SP_CHUNK;
-            if (prepared) {
+            if (route.prepared) {
                 if (n_chunks > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "batch too large for one launch");
                 const int64_t cap_chunks = (pod_headroom(P) + kgpu::SP_CHUNK - 1) / kgpu::SP_CHUNK;
                 KGPU_CUDA(h, s.d_chunks.reserve(n_chunks * kgpu::SP_CHUNK_INT4, cap_chunks * kgpu::SP_CHUNK_INT4));
             }
-            const int4 *d_chunks = prepared ? s.d_chunks.get() : nullptr;
-#define KGPU_PREPARE_CHUNKS(MEMF)                                                                             \
-    if (prepared) {                                                                                           \
-        kgpu::sp_prepare_chunks<MEMF><<<(unsigned)n_chunks, kgpu::SP_THREADS, 0, st>>>(pods4, P, s.d_flag, s.d_chunks); \
-        h->launches++;                                                                                        \
-    }
-            bool byte_keys = true;       // every cost < 2^16 <=> 28 * max weight < 65536
-            for (int i = 0; i < 16; i++) byte_keys = byte_keys && h->W[i] <= 2340;
-#define KGPU_LAUNCH_SPARSE(MEMF, BK, ST)                                                                      \
-    kgpu::score_pairs_sparse<true, MEMF, BK, ST><<<grid, kgpu::SP_THREADS, 0, st>>>(                          \
-        s.d_rec, s.d_meta, s.d_mem, s.d_order, s.d_flag, s.node_id_base, pods4, P, (int)per, d_work, PC, d_keys, d_chunks)
-#define KGPU_LAUNCH_SPARSE_TMA(BK, MB)                                                                        \
-    kgpu::score_pairs_sparse<true, false, BK, true, MB><<<grid, kgpu::SP_THREADS, kgpu::SP_TMA_DYN_SMEM, st>>>(   \
-        s.d_rec, s.d_meta, s.d_mem, s.d_order, s.d_flag, s.node_id_base, pods4, P, (int)per, d_work, PC, d_keys)
-            // few pods (the batch is one chunk): the work list holds runs of tiles -> the STREAM instantiation (next
-            // tile's record prefetched into registers while the current one is scored); at most 64 pods: the TMA one
-            // (tiles staged by cp.async.bulk into shared memory, 7 blocks per SM; KGPU_SP_TMA=0 turns it off)
-            const bool stream_build = use_work && P <= kgpu::kSparseChunk;
-            const bool tma_build = stream_build && tma_mode != 0 && P <= kgpu::SP_TMA_PODS;
-            if (tma_build && !s.tma_attr_done) {   // static + dynamic shared memory may pass 48 KB with more stages: opt in, once per device
-                const int bytes = (int)kgpu::SP_TMA_DYN_SMEM;
-                cudaError_t e = cudaFuncSetAttribute(kgpu::score_pairs_sparse<true, false, true, true, KGPU_SP_TMA_MINBLOCKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-                if (e == cudaSuccess) e = cudaFuncSetAttribute(kgpu::score_pairs_sparse<true, false, false, true, KGPU_SP_TMA_MINBLOCKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+            const int4 *d_chunks = route.prepared ? s.d_chunks.get() : nullptr;
+            if (route.tma && !s.tma_attr_done) {   // static + dynamic shared memory may pass 48 KB with more stages: opt in, once per device
+                kgpu::SparseRoute r = route;
+                r.byte_keys = true;
+                cudaError_t e = cudaFuncSetAttribute(kgpu::sparse_kernel(r, false), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kgpu::SP_TMA_DYN_SMEM);
+                r.byte_keys = false;
+                if (e == cudaSuccess) e = cudaFuncSetAttribute(kgpu::sparse_kernel(r, false), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kgpu::SP_TMA_DYN_SMEM);
                 if (e != cudaSuccess) return fail(h, KGPU_ERR_CUDA, "cudaFuncSetAttribute(TMA K1s): %s", cudaGetErrorString(e));
                 s.tma_attr_done = true;
             }
-            if (sparse_main) {
-                if (tma_build) { if (byte_keys) KGPU_LAUNCH_SPARSE_TMA(true, KGPU_SP_TMA_MINBLOCKS); else KGPU_LAUNCH_SPARSE_TMA(false, KGPU_SP_TMA_MINBLOCKS); }
-                else if (stream_build) { if (byte_keys) KGPU_LAUNCH_SPARSE(false, true, true); else KGPU_LAUNCH_SPARSE(false, false, true); }
-                else {
-                    KGPU_PREPARE_CHUNKS(false)
-                    if (byte_keys) KGPU_LAUNCH_SPARSE(false, true, false); else KGPU_LAUNCH_SPARSE(false, false, false);
+            auto launch = [&](bool mem) {
+                if (route.prepared) {
+                    if (mem) kgpu::sp_prepare_chunks<true><<<(unsigned)n_chunks, kgpu::SP_THREADS, 0, st>>>(pods4, P, s.d_flag, s.d_chunks);
+                    else kgpu::sp_prepare_chunks<false><<<(unsigned)n_chunks, kgpu::SP_THREADS, 0, st>>>(pods4, P, s.d_flag, s.d_chunks);
+                    h->launches++;
                 }
+                const kgpu::SparseKernel k1s = kgpu::sparse_kernel(route, mem);
+                k1s<<<grid, kgpu::SP_THREADS, route.tma && !mem ? kgpu::SP_TMA_DYN_SMEM : 0, st>>>(
+                    s.d_rec, s.d_meta, s.d_mem, s.d_order, s.d_flag, s.node_id_base, pods4, P, (int)per, d_work, PC, d_keys, d_chunks);
                 h->launches++;
-            }
-            if (has_mem != 0) {
-                KGPU_PREPARE_CHUNKS(true)
-                if (byte_keys) KGPU_LAUNCH_SPARSE(true, true, false); else KGPU_LAUNCH_SPARSE(true, false, false);
-                h->launches++;
-            }
-#undef KGPU_PREPARE_CHUNKS
-#undef KGPU_LAUNCH_SPARSE
-#undef KGPU_LAUNCH_SPARSE_TMA
+            };
+            if (sparse_main) launch(false);
+            if (has_mem != 0) launch(true);
         } else if (has_mem != 0) {   // K1m: the memory-constrained pods (its blocks exit at once if the flag is 0)
             kgpu::score_pairs_lane_per_node<true, true><<<grid, kgpu::LPN_THREADS, 0, st>>>(
                 topo4, s.d_free, mem4, s.d_flag, s.n, s.node_id_base, pods4, P, (int)per, W, PC, d_keys);
@@ -869,20 +833,9 @@ int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, i
         const int rc = check_gang_runs(h, "kgpu_place_batch_gang", gang, P);
         if (rc != KGPU_OK) return rc;
     }
-    // the batch's distinct memory requirements are the views the sequential kernels keep tables for
     kgpu::PlaceViews views;
-    memset(&views, 0, sizeof views);
-    views.n = 1;
-    for (int64_t p = 0; p < P; p++) {
-        const int32_t need = pods[4 * p + 3];
-        if (need <= 0 || pods[4 * p] < 0 || pods[4 * p] > 8) continue;
-        bool seen = false;
-        for (int j = 1; j < views.n; j++) seen = seen || views.min_mem[j] == need;
-        if (seen) continue;
-        if (views.n == kgpu::PLACE_MAX_VIEWS)
-            return fail(h, KGPU_ERR_INVALID, "kgpu_place_batch: more than %d distinct min_mem values in one batch", kgpu::PLACE_MAX_VIEWS - 1);
-        views.min_mem[views.n++] = need;
-    }
+    if (!kgpu::place_views(pods, P, views))
+        return fail(h, KGPU_ERR_INVALID, "kgpu_place_batch: more than %d distinct min_mem values in one batch", kgpu::PLACE_MAX_VIEWS - 1);
     kgpu_shard &s = h->shards[0];
     const int rc = reserve_pods(h, s, P);
     if (rc != KGPU_OK) return rc;
@@ -912,17 +865,16 @@ int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, i
         kgpu::place_half_tables<<<(unsigned)std::min<int64_t>((s.n + 3) / 4, (int64_t)s.sm_count * 16), 128, 0, s.stream>>>(
             s.d_topo, s.n, W, s.d_half);
         h->launches++;
+        if (!s.place_attr_done) {          // 72 KB of dynamic shared memory: opt in, once per device
+            KGPU_CUDA(h, cudaFuncSetAttribute(kgpu::place_sequential<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kgpu::PLACE_DYN_SMEM));
+            KGPU_CUDA(h, cudaFuncSetAttribute(kgpu::place_sequential<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kgpu::PLACE_DYN_SMEM));
+            s.place_attr_done = true;
+        }
         if (gang) {
-            static const cudaError_t place_gang_attr = cudaFuncSetAttribute(
-                kgpu::place_sequential<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kgpu::PLACE_DYN_SMEM);
-            KGPU_CUDA(h, place_gang_attr);
             kgpu::place_sequential<true><<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(
                 s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base, reinterpret_cast<const int4 *>(s.d_pods.get()), P, W, views,
                 s.d_nodebest, s.d_tilebest, T, s.d_half, s.d_keys, s.d_gang);
         } else {
-            static const cudaError_t place_attr = cudaFuncSetAttribute(kgpu::place_sequential<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                                       (int)kgpu::PLACE_DYN_SMEM);
-            KGPU_CUDA(h, place_attr);
             kgpu::place_sequential<false><<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base,
                                                                                    reinterpret_cast<const int4 *>(s.d_pods.get()), P, W, views,
                                                                                    s.d_nodebest, s.d_tilebest, T, s.d_half, s.d_keys);
@@ -1092,41 +1044,19 @@ int kgpu_preempt_batch(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64
 }
 
 namespace {
-// kgpu_preempt_plan[_gang]: the batch's checks and its columns, the distinct (k, level, min_mem) with k in 1..8, sorted
-// (k first, so warps stay on one k); pcol[p] = pod p's column, -1 for k outside 1..8.
+// kgpu_preempt_plan[_gang]: the batch's checks and its columns (launch_plan.h)
 int plan_columns(kgpu_ctx *h, const char *fn, const int32_t *pods, const int32_t *lvl, int64_t P, std::vector<int4> &cols,
                  std::vector<int32_t> &pcol) {
     for (int64_t p = 0; p < P; p++)
         if (lvl[p] < 0 || lvl[p] > 15) return fail(h, KGPU_ERR_INVALID, "%s: lvl[%lld] = %d outside 0..15", fn, (long long)p, lvl[p]);
     if (P > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "%s: more than 2^31 pods", fn);
-    std::vector<std::array<int32_t, 3>> trip;
-    std::vector<int32_t> mems;
-    std::vector<std::pair<int32_t, int32_t>> views;      // (level, min_mem) with level > 0
-    for (int64_t p = 0; p < P; p++) {
-        const int32_t k = pods[4 * p], need = std::max<int32_t>(0, pods[4 * p + 3]);
-        if (k < 0 || k > 8) continue;
-        if (need > 0) mems.push_back(need);
-        if (lvl[p] > 0) views.push_back({lvl[p], need});
-        if (k > 0) trip.push_back({k, lvl[p], need});
-    }
-    std::sort(trip.begin(), trip.end());
-    trip.erase(std::unique(trip.begin(), trip.end()), trip.end());
-    std::sort(mems.begin(), mems.end());
-    mems.erase(std::unique(mems.begin(), mems.end()), mems.end());
-    std::sort(views.begin(), views.end());
-    views.erase(std::unique(views.begin(), views.end()), views.end());
-    if (mems.size() > (size_t)kgpu::PLACE_MAX_VIEWS - 1)
-        return fail(h, KGPU_ERR_INVALID, "%s: more than %d distinct min_mem values in one batch", fn, kgpu::PLACE_MAX_VIEWS - 1);
-    if (views.size() > 32) return fail(h, KGPU_ERR_INVALID, "%s: more than 32 distinct (level > 0, min_mem) pairs in one batch", fn);
-    const int ncol = (int)trip.size();           // <= 8 k x (8 level-0 + 32 other views) = PLAN_MAX_COLS
-    cols.resize((size_t)ncol);
-    for (int c = 0; c < ncol; c++) cols[(size_t)c] = make_int4(trip[(size_t)c][0], trip[(size_t)c][1], trip[(size_t)c][2], 0);
-    pcol.assign((size_t)P, -1);
-    for (int64_t p = 0; p < P; p++) {
-        const int32_t k = pods[4 * p];
-        if (k < 1 || k > 8) continue;
-        const std::array<int32_t, 3> t = {k, lvl[p], std::max<int32_t>(0, pods[4 * p + 3])};
-        pcol[(size_t)p] = (int32_t)(std::lower_bound(trip.begin(), trip.end(), t) - trip.begin());
+    switch (kgpu::plan_columns(pods, lvl, P, cols, pcol)) {
+        case kgpu::PlanColumns::too_many_min_mem:
+            return fail(h, KGPU_ERR_INVALID, "%s: more than %d distinct min_mem values in one batch", fn, kgpu::PLACE_MAX_VIEWS - 1);
+        case kgpu::PlanColumns::too_many_views:
+            return fail(h, KGPU_ERR_INVALID, "%s: more than 32 distinct (level > 0, min_mem) pairs in one batch", fn);
+        case kgpu::PlanColumns::ok:
+            break;
     }
     if (h->shards[0].n > 0x7FFFFFFFLL) return fail(h, KGPU_ERR_INVALID, "%s: too many nodes for the key's node field", fn);
     return KGPU_OK;

@@ -1,0 +1,132 @@
+// launch_plan.h -- the host-side plans around libkgpu's launches, written once: kgpu.cu launches what they say on the
+// device and the CPU emulation of the tests (tests/emu) launches the same on the CPU.  Host code only, no CUDA runtime
+// calls; it names the kernels' constants, so it comes after their headers.
+#pragma once
+#include <algorithm>
+#include <array>
+#include <cstdint>
+#include <cstring>
+#include <utility>
+#include <vector>
+
+#include "place_sequential.cuh"
+#include "score_pairs_sparse.cuh"
+#include "sparse_work.h"
+
+namespace kgpu {
+
+// c_subsets / c_nsub: the k-subsets of the eight GPUs in increasing mask order, for k = 0..8
+inline void subset_tables(uint8_t subs[9][70], uint8_t nsub[9]) {
+    std::memset(subs, 0, 9 * 70);
+    for (int k = 0; k <= 8; k++) {
+        int c = 0;
+        for (unsigned S = 0; S < 256; S++)
+            if (__builtin_popcount(S) == k) subs[k][c++] = (uint8_t)S;
+        nsub[k] = (uint8_t)c;
+    }
+}
+
+// K3: the batch's distinct memory requirements are the views the sequential kernels keep tables for (view 0: none).
+// False when there are more than PLACE_MAX_VIEWS - 1 of them.
+inline bool place_views(const int32_t *pods, int64_t P, PlaceViews &views) {
+    std::memset(&views, 0, sizeof views);
+    views.n = 1;
+    for (int64_t p = 0; p < P; p++) {
+        const int32_t need = pods[4 * p + 3];
+        if (need <= 0 || pods[4 * p] < 0 || pods[4 * p] > 8) continue;
+        bool seen = false;
+        for (int j = 1; j < views.n; j++) seen = seen || views.min_mem[j] == need;
+        if (seen) continue;
+        if (views.n == PLACE_MAX_VIEWS) return false;
+        views.min_mem[views.n++] = need;
+    }
+    return true;
+}
+
+// Preemption plans: the batch's columns, the distinct (k, level, min_mem) with k in 1..8, sorted (k first, so warps stay
+// on one k); pcol[p] = pod p's column, -1 for k outside 1..8.  lvl must already lie in 0..15.  Both are filled in whatever
+// the status: it says which of libkgpu's limits the batch passes, which keep the columns within PLAN_MAX_COLS.
+enum class PlanColumns { ok, too_many_min_mem, too_many_views };
+inline PlanColumns plan_columns(const int32_t *pods, const int32_t *lvl, int64_t P, std::vector<int4> &cols,
+                                std::vector<int32_t> &pcol) {
+    std::vector<std::array<int32_t, 3>> trip;
+    std::vector<int32_t> mems;
+    std::vector<std::pair<int32_t, int32_t>> views;      // (level, min_mem) with level > 0
+    for (int64_t p = 0; p < P; p++) {
+        const int32_t k = pods[4 * p], need = std::max<int32_t>(0, pods[4 * p + 3]);
+        if (k < 0 || k > 8) continue;
+        if (need > 0) mems.push_back(need);
+        if (lvl[p] > 0) views.push_back({lvl[p], need});
+        if (k > 0) trip.push_back({k, lvl[p], need});
+    }
+    std::sort(trip.begin(), trip.end());
+    trip.erase(std::unique(trip.begin(), trip.end()), trip.end());
+    std::sort(mems.begin(), mems.end());
+    mems.erase(std::unique(mems.begin(), mems.end()), mems.end());
+    std::sort(views.begin(), views.end());
+    views.erase(std::unique(views.begin(), views.end()), views.end());
+    const int ncol = (int)trip.size();           // <= 8 k x (8 level-0 + 32 other views) = PLAN_MAX_COLS
+    cols.resize((size_t)ncol);
+    for (int c = 0; c < ncol; c++) cols[(size_t)c] = make_int4(trip[(size_t)c][0], trip[(size_t)c][1], trip[(size_t)c][2], 0);
+    pcol.assign((size_t)P, -1);
+    for (int64_t p = 0; p < P; p++) {
+        const int32_t k = pods[4 * p];
+        if (k < 1 || k > 8) continue;
+        const std::array<int32_t, 3> t = {k, lvl[p], std::max<int32_t>(0, pods[4 * p + 3])};
+        pcol[(size_t)p] = (int32_t)(std::lower_bound(trip.begin(), trip.end(), t) - trip.begin());
+    }
+    if (mems.size() > (size_t)PLACE_MAX_VIEWS - 1) return PlanColumns::too_many_min_mem;
+    if (views.size() > 32) return PlanColumns::too_many_views;
+    return PlanColumns::ok;
+}
+
+// K1s: the largest free count of every SP_THREADS-slot tile of the order, from the class layout alone: class c's nodes
+// sit in [start, start + count), every class padded to a multiple of `pad` slots, classes 8 first.
+inline std::vector<uint8_t> tile_classes(const int64_t class_count[9], int64_t pad, int64_t n_slots) {
+    std::vector<uint8_t> tc((size_t)(n_slots / SP_THREADS), 0);
+    int64_t start = 0;
+    for (int c = 8; c >= 0; c--) {
+        const int64_t cnt = class_count[c];
+        if (cnt > 0)
+            for (int64_t t = start / SP_THREADS; t <= (start + cnt - 1) / SP_THREADS; t++)
+                tc[(size_t)t] = std::max<uint8_t>(tc[(size_t)t], (uint8_t)c);
+        start += (cnt + pad - 1) / pad * pad;
+    }
+    return tc;
+}
+
+// The byte-aligned warp key of K1s: every cost < 2^16 <=> 28 * max weight < 65536
+inline bool byte_keys(const int32_t *W) {
+    for (int i = 0; i < 16; i++)
+        if (W[i] > 2340) return false;
+    return true;
+}
+
+// Which K1s instantiation runs a batch of P pods.  On the work list (use_work), a batch of one chunk is cut into runs of
+// tiles and goes to the STREAM instantiation (next tile's record prefetched into registers), at most SP_TMA_PODS pods to
+// the TMA one (tiles staged by cp.async.bulk; tma_mode 0 turns it off); a chunk-aligned list takes the chunk tables
+// sp_prepare_chunks builds once per launch, otherwise every block sorts its pods itself.  The MEM launch is never a
+// streaming one.  sparse_kernel (score_pairs_sparse.cuh) names the instantiation.
+inline SparseRoute sparse_route(int64_t P, bool use_work, bool aligned, int tma_mode, const int32_t *W) {
+    SparseRoute r;
+    r.stream = use_work && P <= kSparseChunk;
+    r.tma = r.stream && tma_mode != 0 && P <= SP_TMA_PODS;
+    r.prepared = use_work && aligned;
+    r.byte_keys = byte_keys(W);
+    return r;
+}
+
+// The resident blocks the work list is cut for: those of the instantiation that will run it.
+inline int64_t sparse_list_resident(int64_t P, int tma_mode, int64_t sm_count, int64_t resident) {
+    if (tma_mode != 0 && P <= SP_TMA_PODS) return sm_count * KGPU_SP_TMA_MINBLOCKS;
+    if (P <= kSparseChunk) return sm_count * KGPU_SP_STREAM_MINBLOCKS;
+    return resident;
+}
+
+// Pods per split of a plain (tiles x splits) grid: equal ranges rounded up to whole warps of pods
+inline int64_t pods_per_split(int64_t P, int64_t splits) {
+    const int64_t per = (P + splits - 1) / splits;
+    return (per + 31) / 32 * 32;
+}
+
+}  // namespace kgpu

@@ -750,4 +750,21 @@ score_pairs_sparse(const int4 *__restrict__ rec, const uint32_t *__restrict__ me
     }
 }
 
+// The host's choice of K1s instantiation for a batch (launch_plan.h: sparse_route), and the one kernel it names; mem: the
+// launch for the memory-constrained pods.  Every instantiation takes the same arguments (the streaming ones ignore
+// `chunks`), so libkgpu and the CPU emulation launch whatever this returns.
+struct SparseRoute {
+    bool stream, tma, prepared, byte_keys;
+};
+using SparseKernel = void (*)(const int4 *, const uint32_t *, const int32_t *, const int32_t *, const int *, int64_t,
+                              const int4 *, int64_t, int, const int4 *, PipeConsts, unsigned long long *, const int4 *);
+inline SparseKernel sparse_kernel(const SparseRoute &r, bool mem) {
+    if (mem) return r.byte_keys ? score_pairs_sparse<true, true, true> : score_pairs_sparse<true, true, false>;
+    if (r.tma)
+        return r.byte_keys ? score_pairs_sparse<true, false, true, true, KGPU_SP_TMA_MINBLOCKS>
+                           : score_pairs_sparse<true, false, false, true, KGPU_SP_TMA_MINBLOCKS>;
+    if (r.stream) return r.byte_keys ? score_pairs_sparse<true, false, true, true> : score_pairs_sparse<true, false, false, true>;
+    return r.byte_keys ? score_pairs_sparse<true, false, true> : score_pairs_sparse<true, false, false>;
+}
+
 }  // namespace kgpu

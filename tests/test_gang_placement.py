@@ -1,7 +1,7 @@
 """Gangs in sequential placement (kgpu_place_batch_gang): a run of consecutive pods with the same nonzero gang id is
 placed all or nothing.  CPU: the gang twin (tests/gang_twin/gang_twin.c, built with the oracle) against the deletion
 property and against a gang-by-gang construction on top of the oracle's plain sequential placement, and the emulated
-kernel (place_sequential<true>, tests/gang_twin/emu_gang.cc) against the twin.  GPU: the device path bit-exact against
+kernel (place_sequential<true>, tests/emu) against the twin.  GPU: the device path bit-exact against
 the twin, dry runs, bad ids, and the host mirror's reordering."""
 import ctypes
 import os
@@ -12,14 +12,13 @@ import subprocess
 import numpy as np
 import pytest
 
+import cpu_libs
 from kubegpu_b200 import _lib, synth
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "gang_twin")
 CLI = os.path.join(ROOT, "kubegpu_b200", "lib", "kgpu_sched_cli")
 NO_FIT = np.uint64(0xFFFFFFFFFFFFFFFF)
-_i32p, _u64p = ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_uint64)
 
 
 def _p(a, t=ctypes.c_int32):
@@ -27,17 +26,10 @@ def _p(a, t=ctypes.c_int32):
 
 
 @pytest.fixture(scope="session")
-def twin(tmp_path_factory):
-    """place(topo, free, pods, gang, mem=None, base=0) -> (keys, free_after): gang_twin.c built with the oracle into a
-    temporary directory."""
+def twin():
+    """place(topo, free, pods, gang, mem=None, base=0) -> (keys, free_after): gang_twin.c built with the oracle."""
     from oracle import oracle_b
-    so = str(tmp_path_factory.mktemp("gang_twin") / "libgang_twin.so")
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11", "-pthread", "-shared", "-o", so,
-                           os.path.join(ROOT, "oracle", "oracle_b.c"), os.path.join(SRC, "gang_twin.c")])
-    L = ctypes.CDLL(so)
-    L.gang_twin_place_batch.restype = None
-    L.gang_twin_place_batch.argtypes = [_i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p, ctypes.c_int64,
-                                        _i32p, _u64p]
+    L = cpu_libs.twin("gang")
     W = np.ascontiguousarray(oracle_b.DEFAULT_WEIGHTS, dtype=np.int32)
 
     def place(topo, free, pods, gang, mem=None, base=0):
@@ -255,16 +247,8 @@ def test_gen_gangs_has_failing_and_placed_gangs(twin, oracle_b):
 
 # ---- the kernel on the CPU (tests/emu) -------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    """emu_gang.cc (the kernel source under tests/emu/cuda_emu.h) built into a temporary directory."""
-    so = str(tmp_path_factory.mktemp("gang_emu") / "libgang_emu.so")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I" + os.path.join(HERE, "emu", "stub"),
-                           "-I" + os.path.join(HERE, "emu"), "-I" + os.path.join(ROOT, "kubegpu_b200", "csrc"), "-o", so,
-                           os.path.join(SRC, "emu_gang.cc")])
-    L = ctypes.CDLL(so)
-    L.emu_place_batch_gang.restype = ctypes.c_int
-    L.emu_place_batch_gang.argtypes = [_i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p, ctypes.c_int64, _i32p, _u64p]
-    return L
+def emu():
+    return cpu_libs.emu()
 
 
 def emu_place(emu, topo, free, pods, gang, mem=None, base=0):

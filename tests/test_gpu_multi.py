@@ -39,6 +39,22 @@ def test_multi_device_handle_matches_oracle(oracle_b, G):
         assert (s.score_batch(pods) == oracle_b.score_batch(topo2, free2, pods, node_id_base=17, fast=True, nthreads=8)).all()
 
 
+def test_sequential_placement_on_two_devices_in_one_process(oracle_b):
+    """K3 opts in to its dynamic shared memory per device: single-device handles on devices 0 and 1 of one process both
+    place (plain and gang batches) and match the oracle."""
+    if _ndev() < 2:
+        pytest.skip("needs 2 GPUs")
+    from kubegpu_b200.scorer import Scorer
+    topo, free, pods = synth.gen_c4(N=3000, P=200, seed=5)
+    alone = np.zeros(len(pods), dtype=np.int32)             # gang ids 0: every pod on its own, the plain placement
+    want, want_free = oracle_b.place_batch(topo, free.copy(), pods)
+    with Scorer((0,)) as a, Scorer((1,)) as b:
+        for s in (a, b):
+            s.upload_nodes(topo, free)
+            assert (s.place_batch(pods, dry_run=True, gang=alone) == want).all()
+            assert (s.place_batch(pods) == want).all() and (s.get_free_masks() == want_free).all()
+
+
 def test_torchrun_bench_keys_equal_single_gpu(tmp_path):
     """The one-process-per-GPU path of bench.py (torch.distributed NCCL all-gather + K2): the final
     keys at N=2 must be the very same bits as at N=1 (SURVEY.md 8(e): result independent of G)."""

@@ -5,18 +5,17 @@ memory classes, answer bit-exact against Oracle B and the preemption twin."""
 import ctypes
 import os
 import re
-import subprocess
 
 import numpy as np
 import pytest
 
+import cpu_libs
 from kubegpu_b200 import synth
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(ROOT, "kubegpu_b200", "csrc")
 NO_FIT = np.uint64(0xFFFFFFFFFFFFFFFF)
-_i32p, _u64p, _u32p = ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint32)
 RAW_CALLS = ("cudaMalloc(", "cudaFree(", "cudaMallocHost(", "cudaFreeHost(")
 
 
@@ -48,16 +47,10 @@ def test_allocations_only_in_buffer_type():
 
 # ---- the device path -----------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def preempt_twin(tmp_path_factory):
+def preempt_twin():
     """preempt(topo, free, pods, lvl, hold=None, mem=None) -> (keys, victims): tests/preempt_twin built with the oracle."""
     from oracle import oracle_b
-    so = str(tmp_path_factory.mktemp("preempt_twin") / "libpreempt_twin.so")
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11", "-pthread", "-shared", "-o", so,
-                           os.path.join(ROOT, "oracle", "oracle_b.c"), os.path.join(HERE, "preempt_twin", "preempt_twin.c")])
-    L = ctypes.CDLL(so)
-    L.preempt_twin_batch.restype = None
-    L.preempt_twin_batch.argtypes = [_i32p, _i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p, ctypes.c_int64,
-                                     _i32p, ctypes.c_int, _u64p, _u32p]
+    L = cpu_libs.twin("preempt")
     W = np.ascontiguousarray(oracle_b.DEFAULT_WEIGHTS, dtype=np.int32)
 
     def preempt(topo, free, pods, lvl, hold=None, mem=None):

@@ -1,18 +1,15 @@
-"""K1s's per-launch chunk tables on the CPU (tests/k1s_chunks/emu_chunks.cc, the kernels compiled against tests/emu):
+"""K1s's per-launch chunk tables on the CPU (the kernels compiled against tests/emu):
 sp_prepare_chunks builds every 512-pod chunk's sorted pod table once per launch, and the K1s blocks of a chunk-aligned
 work list copy it instead of sorting.  Checked here: both tables against an independent Python layout, the keys of the
 prepared path against Oracle B and the in-kernel path, and the work-list rule that decides between them."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import cpu_libs
 from kubegpu_b200 import synth
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 CHUNK = 512
 DUMMY = 0xFFFF
 WEIGHTS = {"default": None, "flat_max": [4095] * 16}
@@ -23,16 +20,8 @@ def _p(a, t=ctypes.c_int32):
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("k1s_chunks") / "libk1s_chunks.so")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I" + os.path.join(HERE, "emu", "stub"),
-                           "-I" + os.path.join(HERE, "emu"), "-I" + os.path.join(ROOT, "kubegpu_b200", "csrc"), "-o", so,
-                           os.path.join(HERE, "k1s_chunks", "emu_chunks.cc")])
-    L = ctypes.CDLL(so)
-    L.emu_chunk_tables.restype = ctypes.c_int64
-    L.emu_score_chunks.restype = ctypes.c_int
-    L.emu_work_list.restype = ctypes.c_int64
-    return L
+def emu():
+    return cpu_libs.emu()
 
 
 def _pods(P, seed, mem_share=0.3):
@@ -143,8 +132,8 @@ def test_work_list_chunk_alignment(emu, tiles, aligned):
     tile_class = np.sort(rng.integers(0, 9, size=tiles).astype(np.uint8))[::-1].copy()
     out = np.zeros((200_000, 4), np.int32)
     flag = ctypes.c_int(-1)
-    n = emu.emu_work_list(_p(tile_class, ctypes.c_uint8), ctypes.c_int64(tiles), ctypes.c_int64(P), ctypes.c_int64(resident),
-                          _p(out), ctypes.c_int64(len(out)), ctypes.byref(flag))
+    n = emu.emu_sparse_work(_p(tile_class, ctypes.c_uint8), ctypes.c_int64(tiles), ctypes.c_int64(P), ctypes.c_int64(resident),
+                            _p(out), ctypes.c_int64(len(out)), None, ctypes.byref(flag))
     items = out[:n]
     assert flag.value == int(aligned)
     assert (items[:, 3] == 1).all()

@@ -3,27 +3,17 @@ small CUDA shim (tests/emu/cuda_emu.h: one OS thread per CUDA thread, real barri
 collectives) and run on the CPU against the oracle.  Small sizes only -- this is a logic check that works
 without a GPU (e.g. for kernel edits between GPU runs); bit-exactness on the H100 is tests/test_gpu_*.py."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import cpu_libs
 from kubegpu_b200 import synth
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-LIB = os.path.join(HERE, "emu", "_build", "libkgpu_emu.so")
 
 
 @pytest.fixture(scope="module")
 def emu():
-    subprocess.check_call(["make", "-s", "-C", os.path.join(HERE, "emu")])
-    L = ctypes.CDLL(LIB)
-    i32p, u64p = ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_uint64)
-    for fn in (L.emu_score_sparse, L.emu_score_dense):
-        fn.restype = None
-        fn.argtypes = [i32p, i32p, i32p, ctypes.c_int64, ctypes.c_int64, i32p, ctypes.c_int64, i32p, ctypes.c_int, u64p]
-    return L
+    return cpu_libs.emu()
 
 
 def _run(fn, topo, free, pods, W, mem=None, base=0, splits=1):
@@ -71,7 +61,6 @@ def _p(a, t=ctypes.c_int32):
 @pytest.mark.parametrize("variant", [1, 3, 4])
 def test_emulated_other_variants_match_oracle(emu, oracle_b, variant):
     """warp-per-pair (the north_star mapping), memo-by-k and tile-memo, incl. their memory-aware routes."""
-    emu.emu_score_variant.restype = None
     W = np.ascontiguousarray(oracle_b.DEFAULT_WEIGHTS, dtype=np.int32)
     topo, free, mem, pods = synth.gen_c6(N=200, P=40)
     pods[3, 0], pods[4, 0] = 0, 11
@@ -87,7 +76,6 @@ def test_emulated_other_variants_match_oracle(emu, oracle_b, variant):
 
 
 def test_emulated_reduce_shards(emu, oracle_b):
-    emu.emu_reduce_shards.restype = None
     rng = np.random.default_rng(5)
     g = rng.integers(0, 2**63, size=(4, 300), dtype=np.uint64)
     g[:, 7] = np.uint64(0xFFFFFFFFFFFFFFFF)
@@ -97,7 +85,6 @@ def test_emulated_reduce_shards(emu, oracle_b):
 
 
 def test_emulated_pair_list(emu, oracle_b):
-    emu.emu_score_pair_list.restype = None
     W = np.ascontiguousarray(oracle_b.DEFAULT_WEIGHTS, dtype=np.int32)
     topo, free, mem, pods = synth.gen_c6(N=150, P=150)
     rng = np.random.default_rng(6)
@@ -114,7 +101,6 @@ def test_emulated_pair_list(emu, oracle_b):
 
 
 def _place(emu, topo, free, pods, W, mem=None, base=0):
-    emu.emu_place_batch.restype = ctypes.c_int
     f = np.ascontiguousarray(free, dtype=np.int32).copy()
     pods = np.ascontiguousarray(pods, dtype=np.int32)
     keys = np.empty(len(pods), dtype=np.uint64)
@@ -192,14 +178,13 @@ def test_emulated_sparse_work_list(emu, oracle_b):
 def test_sparse_work_list_partitions_the_tile_pod_plane(emu, P, resident):
     """Every (tile, pod) cell is covered exactly once; items come heaviest first; pod ranges start on multiples of
     32; runs of several tiles only when the whole batch fits one chunk of the block's pod sort."""
-    emu.emu_sparse_work.restype = ctypes.c_int64
     rng = np.random.default_rng(P + resident)
     ntile = 57 if P > 512 else 700
     tile_class = np.sort(rng.integers(0, 9, size=ntile).astype(np.uint8))[::-1].copy()      # the order puts class 8 first
     out = np.zeros((200_000, 4), dtype=np.int32)
     weight = np.zeros(200_000, dtype=np.int64)
     n = emu.emu_sparse_work(_p(tile_class, ctypes.c_uint8), ctypes.c_int64(ntile), ctypes.c_int64(P), ctypes.c_int64(resident),
-                            _p(out), ctypes.c_int64(len(out)), _p(weight, ctypes.c_longlong))
+                            _p(out), ctypes.c_int64(len(out)), _p(weight, ctypes.c_longlong), None)
     items, weight = out[:n], weight[:n]
     assert 1 <= n <= len(out)
     assert (np.diff(weight) <= 0).all() and (weight > 0).all()                     # heaviest first
@@ -255,7 +240,6 @@ def test_emulated_gather_and_min_single_rank(emu):
     the local key array is left at NO_FIT for the next step's K1, the last block resets the ticket and publishes the epoch;
     P = 0 is a pure barrier.  (One block only: the emulation runs blocks one after the other, and every block of
     this kernel waits for the flag its rank's LAST block publishes -- on the GPU all blocks are resident.)"""
-    emu.emu_gather_and_min.restype = None
     P, MP = 250, 1000
     rng = np.random.default_rng(3)
     local = rng.integers(1, 2**60, size=P, dtype=np.uint64)
@@ -300,7 +284,6 @@ def test_emulated_device_order_is_the_stable_class_sort(emu, n):
     order = np.empty(cap, dtype=np.int32)
     slot_of = np.empty(n, dtype=np.int32)
     cc = np.zeros(9, dtype=np.int64)
-    emu.emu_order.restype = ctypes.c_int64
     n_slots = emu.emu_order(_p(free), ctypes.c_int64(n), _p(order), ctypes.c_int64(cap), _p(slot_of), _p(cc, ctypes.c_longlong))
     assert n_slots == len(want)
     assert (order[:n_slots] == want).all() and (order[n_slots:] == -1).all()
@@ -323,7 +306,6 @@ def test_emulated_incremental_mask_updates_equal_fresh_upload(emu, oracle_b):
     for splits in (1, 2):
         keys = np.empty(len(pods), dtype=np.uint64)
         out_free = np.empty_like(free0)
-        emu.emu_score_sparse_after_updates.restype = None
         emu.emu_score_sparse_after_updates(_p(np.ascontiguousarray(topo, dtype=np.int32)), _p(free0), ctypes.c_int64(len(free0)),
                                            _p(upd_idx), _p(upd_mask), ctypes.c_int64(len(upd_idx)), _p(pods), ctypes.c_int64(len(pods)),
                                            _p(np.ascontiguousarray(W, dtype=np.int32)), splits, _p(keys, ctypes.c_uint64), _p(out_free))
@@ -335,7 +317,6 @@ def test_emulated_fit_table_rows(emu, oracle_b):
     W = np.ascontiguousarray(oracle_b.DEFAULT_WEIGHTS, dtype=np.int32)
     topo, free, _ = synth.gen_c4(N=200, P=1)
     topo = np.ascontiguousarray(topo, dtype=np.int32)
-    emu.emu_fit_nodes.restype = None
     out = np.empty(9 * 200, dtype=np.uint32)
     emu.emu_fit_nodes(_p(topo), _p(free), ctypes.c_int64(200), None, ctypes.c_int64(200), _p(W), _p(out, ctypes.c_uint32))
     for i in range(0, 200, 7):
@@ -352,7 +333,6 @@ def test_emulated_fit_table_rows(emu, oracle_b):
 def test_emulated_validate_topo(emu):
     topo, _, _ = synth.gen_c4(N=100, P=1)
     topo = np.ascontiguousarray(topo, dtype=np.int32)
-    emu.emu_validate_topo.restype = ctypes.c_longlong
     assert emu.emu_validate_topo(_p(topo), ctypes.c_int64(100)) == -1
     topo[40, 9] = 16
     topo[77, 3] = -1
@@ -395,3 +375,41 @@ def test_emulated_few_pod_instantiations_at_their_boundaries(emu, oracle_b, P, w
     want = oracle_b.score_batch(topo, free, pods, W, node_id_base=11)
     for resident in (1, 2):                                   # runs of many tiles / of a few tiles per item
         assert (_run(emu.emu_score_sparse, topo, free, pods, W, base=11, splits=-resident) == want).all(), resident
+
+
+@pytest.mark.parametrize("pad", [32, 128])
+def test_tile_classes_from_class_counts_equal_slot_maxima(emu, pad):
+    """The hosts derive each tile's class from the order's class counts alone (launch_plan.h: tile_classes); that must be
+    the largest free count among the tile's nodes, with classes padded to warps (32) or to whole tiles (128)."""
+    rng = np.random.default_rng(pad)
+    for n in (1, 127, 1000, 3333):
+        free = (rng.integers(0, 256, size=n) & rng.integers(0, 256, size=n)).astype(np.int32)
+        if n == 1000:
+            free[rng.random(n) < 0.5] = 0xFF
+        cap = (n + 11 * 128) // 128
+        got, want = np.zeros(cap, np.uint8), np.zeros(cap, np.uint8)
+        tiles = emu.emu_tile_classes(_p(free), n, pad, _p(got, ctypes.c_uint8), _p(want, ctypes.c_uint8), cap)
+        assert 1 <= tiles <= cap
+        assert (got[:tiles] == want[:tiles]).all(), n
+
+
+K1S_ROUTES = {"in_block_sort": 0, "prepared": 1, "stream": 2, "tma": 3}
+
+
+@pytest.mark.parametrize("route", sorted(K1S_ROUTES))
+@pytest.mark.parametrize("mem", [False, True])
+@pytest.mark.parametrize("byte_keys", [True, False])
+def test_emulated_k1s_routes(emu, oracle_b, route, mem, byte_keys):
+    """Each K1s route the host plan can pick (TMA, STREAM, prepared chunk tables, the blocks' own pod sort), with and without
+    the MEM launch and byte keys, is reached (emu_score_sparse reports the route it took) and gives Oracle B's keys."""
+    P, splits = {"tma": (40, -1), "stream": (300, -1), "prepared": (600, -1), "in_block_sort": (600, -1184)}[route]
+    topo, free, gmem, pods = synth.gen_c6(N=300, P=P, seed=P)
+    pods[2, 0], pods[3, 0] = 0, 9
+    if not mem:
+        pods[:, 3] = 0
+    W = np.array([(2340 if byte_keys else 2341) - 5 * i for i in range(16)], dtype=np.int32)
+    want = oracle_b.score_batch(topo, free, pods, W, node_id_base=5, mem=gmem, fast=True, nthreads=4)
+    keys = np.empty(P, dtype=np.uint64)
+    got = emu.emu_score_sparse(_p(topo), _p(free), _p(gmem), len(free), 5, _p(pods), P, _p(W), splits, _p(keys, ctypes.c_uint64))
+    assert got == K1S_ROUTES[route] | (4 if mem else 0) | (8 if byte_keys else 0)
+    assert (keys == want).all()

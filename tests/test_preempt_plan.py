@@ -1,7 +1,7 @@
 """Preemption plans (kgpu_preempt_plan): pods in order, each evicting only victims no earlier pod has claimed.
 CPU: a literal reference (a loop of single-pod preempt_twin_batch calls plus the update of the definition) against the
 fast sequential twin (tests/preempt_plan_twin/plan_twin.c), the properties of the definition, the emulated kernels
-(tests/preempt_plan_twin/emu_plan.cc) against the twin, and the kernels' resource usage.  GPU: the device path bit-exact
+(tests/emu) against the twin, and the kernels' resource usage.  GPU: the device path bit-exact
 against the twin on gen_preempt at C2's size and on C3's cluster, the equalities with preempt_batch and dry-run
 placement, rejected batches, and the handle's state left alone."""
 import ctypes
@@ -13,16 +13,14 @@ import subprocess
 import numpy as np
 import pytest
 
+import cpu_libs
 from kubegpu_b200 import _lib, synth
 from test_preemption import _row, random_holders
 from test_weight_tables import TABLES, W_of, edge_matrix
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "preempt_plan_twin")
 NO_FIT = np.uint64(0xFFFFFFFFFFFFFFFF)
-_i32p, _u64p, _u32p = ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint32)
-_ARGS = [_i32p, _i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p, ctypes.c_int64, _i32p]
 
 
 def _p(a, t=ctypes.c_int32):
@@ -39,16 +37,9 @@ def _W(W):
 
 
 @pytest.fixture(scope="session")
-def twins(tmp_path_factory):
+def twins():
     """(snapshot, plan): both (topo, free, pods, lvl, hold=None, mem=None, base=0, W=None) -> (keys, victims)."""
-    so = str(tmp_path_factory.mktemp("plan_twin") / "libplan_twin.so")
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11", "-pthread", "-shared", "-o", so,
-                           os.path.join(ROOT, "oracle", "oracle_b.c"), os.path.join(HERE, "preempt_twin", "preempt_twin.c"),
-                           os.path.join(SRC, "plan_twin.c")])
-    L = ctypes.CDLL(so)
-    for fn in (L.preempt_twin_batch, L.preempt_plan_twin):
-        fn.restype = None
-        fn.argtypes = _ARGS + [ctypes.c_int, _u64p, _u32p]
+    L = cpu_libs.twin("preempt_plan")
 
     def wrap(fn):
         def call(topo, free, pods, lvl, hold=None, mem=None, base=0, W=None):
@@ -249,15 +240,8 @@ def test_case_claims(twins):
 
 # ---- the kernels on the CPU (tests/emu) -------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("plan_emu") / "libplan_emu.so")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I" + os.path.join(HERE, "emu", "stub"),
-                           "-I" + os.path.join(HERE, "emu"), "-I" + os.path.join(ROOT, "kubegpu_b200", "csrc"), "-o", so,
-                           os.path.join(SRC, "emu_plan.cc")])
-    L = ctypes.CDLL(so)
-    L.emu_preempt_plan.restype = ctypes.c_int
-    L.emu_preempt_plan.argtypes = _ARGS + [_u64p, _u32p]
-    return L
+def emu():
+    return cpu_libs.emu()
 
 
 def emu_plan(emu, topo, free, pods, lvl, hold, mem=None, base=0, W=None):

@@ -2,7 +2,7 @@
 CPU: the fast twin (tests/preempt_plan_gang_twin/plan_gang_twin.c) against a literal reference (single-pod
 preempt_twin_batch calls, the update of the definition and an explicit save/restore undo), its properties (the deletion
 property, failed gangs really miss, the equalities with preempt_plan_twin and with K3's gang twin), the emulated kernel
-(tests/preempt_plan_gang_twin/emu_plan_gang.cc) against the twin on named cases, and the build products.  GPU: the device
+(tests/emu) against the twin on named cases, and the build products.  GPU: the device
 path bit-exact against the twin on gen_preempt_gangs and C3's cluster, the deletion property and equalities on the
 device, rejected batches, and a CLI transcript."""
 import ctypes
@@ -14,39 +14,22 @@ import subprocess
 import numpy as np
 import pytest
 
+import cpu_libs
 from kubegpu_b200 import _lib, synth
-from test_preempt_plan import (NO_FIT, _W, _i32p, _opt, _p, _u32p, _u64p, apply_update, big_k_case, check_properties,
-                               random_case, tiles_case, views_32_case)
+from test_preempt_plan import (NO_FIT, _W, _opt, _p, apply_update, big_k_case, check_properties, random_case, tiles_case,
+                               views_32_case)
 from test_preemption import _row, random_holders
 from test_weight_tables import W_of
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "preempt_plan_gang_twin")
-_ARGS = [_i32p, _i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p]
 
 
 @pytest.fixture(scope="session")
-def twins(tmp_path_factory):
+def twins():
     """(snapshot, plan, gang_plan, k3_gang): the single-pod snapshot twin, preempt_plan_twin, preempt_plan_gang_twin and
     K3's gang twin (keys of dry-run gang placement)."""
-    d = tmp_path_factory.mktemp("plan_gang_twin")
-    so = str(d / "libplan_gang_twin.so")
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11", "-pthread", "-shared", "-o", so,
-                           os.path.join(ROOT, "oracle", "oracle_b.c"), os.path.join(HERE, "preempt_twin", "preempt_twin.c"),
-                           os.path.join(SRC, "plan_gang_twin.c")])
-    k3so = str(d / "libgang_twin.so")
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11", "-shared", "-o", k3so,
-                           os.path.join(ROOT, "oracle", "oracle_b.c"), os.path.join(HERE, "gang_twin", "gang_twin.c")])
-    L, K3 = ctypes.CDLL(so), ctypes.CDLL(k3so)
-    for fn in (L.preempt_twin_batch, L.preempt_plan_twin):
-        fn.restype = None
-        fn.argtypes = _ARGS + [ctypes.c_int64, _i32p, ctypes.c_int, _u64p, _u32p]
-    L.preempt_plan_gang_twin.restype = None
-    L.preempt_plan_gang_twin.argtypes = _ARGS + [_i32p, ctypes.c_int64, _i32p, ctypes.c_int, _u64p, _u32p]
-    K3.gang_twin_place_batch.restype = None
-    K3.gang_twin_place_batch.argtypes = [_i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p, ctypes.c_int64,
-                                         _i32p, _u64p]
+    L, K3 = cpu_libs.twin("preempt_plan_gang"), cpu_libs.twin("gang")
 
     def prep(topo, free, pods, lvl):
         return (np.ascontiguousarray(a, dtype=np.int32) for a in (topo, free, pods, lvl))
@@ -287,15 +270,8 @@ def test_case_claims(twins):
 
 # ---- the kernel on the CPU (tests/emu) -------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("plan_gang_emu") / "libplan_gang_emu.so")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I" + os.path.join(HERE, "emu", "stub"),
-                           "-I" + os.path.join(HERE, "emu"), "-I" + os.path.join(ROOT, "kubegpu_b200", "csrc"), "-o", so,
-                           os.path.join(SRC, "emu_plan_gang.cc")])
-    L = ctypes.CDLL(so)
-    L.emu_preempt_plan_gang.restype = ctypes.c_int
-    L.emu_preempt_plan_gang.argtypes = _ARGS + [_i32p, ctypes.c_int64, _i32p, _u64p, _u32p]
-    return L
+def emu():
+    return cpu_libs.emu()
 
 
 def emu_gang_plan(emu, topo, free, pods, lvl, gang, hold, mem=None, base=0, W=None):

@@ -1,6 +1,6 @@
 """Preemption (kgpu_preempt_batch): for pods that fit nowhere, the node, GPUs and lowest-priority running pods to evict.
 CPU: the twin (tests/preempt_twin/preempt_twin.c, built with the oracle) against an independent Python brute force,
-the emulated kernels (tests/preempt_twin/emu_preempt.cc) against the twin, and the kernel's resource usage.  GPU: the
+the emulated kernels (tests/emu) against the twin, and the kernel's resource usage.  GPU: the
 device path bit-exact against the twin on gen_preempt at C2's size, the equalities with score_batch, table updates and
 resets, rejected tables, and the host mirror's victims by name."""
 import ctypes
@@ -13,14 +13,13 @@ import subprocess
 import numpy as np
 import pytest
 
+import cpu_libs
 from kubegpu_b200 import _lib, synth
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "preempt_twin")
 CLI = os.path.join(ROOT, "kubegpu_b200", "lib", "kgpu_sched_cli")
 NO_FIT = np.uint64(0xFFFFFFFFFFFFFFFF)
-_i32p, _u64p, _u32p = ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint32)
 
 
 def _p(a, t=ctypes.c_int32):
@@ -32,16 +31,10 @@ def _opt(a):
 
 
 @pytest.fixture(scope="session")
-def twin(tmp_path_factory):
+def twin():
     """preempt(topo, free, pods, lvl, hold=None, mem=None, base=0) -> (keys, victims)."""
     from oracle import oracle_b
-    so = str(tmp_path_factory.mktemp("preempt_twin") / "libpreempt_twin.so")
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11", "-pthread", "-shared", "-o", so,
-                           os.path.join(ROOT, "oracle", "oracle_b.c"), os.path.join(SRC, "preempt_twin.c")])
-    L = ctypes.CDLL(so)
-    L.preempt_twin_batch.restype = None
-    L.preempt_twin_batch.argtypes = [_i32p, _i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p, ctypes.c_int64,
-                                     _i32p, ctypes.c_int, _u64p, _u32p]
+    L = cpu_libs.twin("preempt")
     W = np.ascontiguousarray(oracle_b.DEFAULT_WEIGHTS, dtype=np.int32)
 
     def preempt(topo, free, pods, lvl, hold=None, mem=None, base=0):
@@ -130,16 +123,8 @@ def test_twin_without_holders_is_score_batch(twin, oracle_b):
 
 # ---- the kernels on the CPU (tests/emu) -------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("preempt_emu") / "libpreempt_emu.so")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I" + os.path.join(HERE, "emu", "stub"),
-                           "-I" + os.path.join(HERE, "emu"), "-I" + os.path.join(ROOT, "kubegpu_b200", "csrc"), "-o", so,
-                           os.path.join(SRC, "emu_preempt.cc")])
-    L = ctypes.CDLL(so)
-    L.emu_preempt_batch.restype = ctypes.c_int
-    L.emu_preempt_batch.argtypes = [_i32p, _i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p, ctypes.c_int64,
-                                    _i32p, ctypes.c_int, _u64p, _u32p]
-    return L
+def emu():
+    return cpu_libs.emu()
 
 
 def emu_preempt(emu, topo, free, pods, lvl, hold, mem=None, base=0, splits=1):

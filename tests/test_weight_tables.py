@@ -12,20 +12,17 @@ handle."""
 import ctypes
 import itertools
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import cpu_libs
 from kubegpu_b200 import _lib, synth
 from test_gang_placement import chunk_batch, edge_batch, random_gangs, runs
 from test_preemption import extreme_levels_case, min_mem_case, multi_block_case, random_holders, ties_case
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 NO_FIT = np.uint64(0xFFFFFFFFFFFFFFFF)
 NODE_NO_FIT = 0xFFFFFFFF
-_i32p, _u64p, _u32p = ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint32)
 
 L_EDGE = 9                                  # an NVLink level of gen_c4 (7..12): the level general_edge and one_level raise
 _rng = np.random.default_rng(0x5EED)
@@ -216,23 +213,11 @@ def ref_preempt(topo, free, pods, lvl, hold, W, mem=None, base=0):
 
 # ---- the twins, with the table as a parameter ---------------------------------------------------------------------------
 @pytest.fixture(scope="session")
-def twins(tmp_path_factory):
+def twins():
     """(gang(topo, free, pods, gang, W, mem=None, base=0) -> (keys, free_after),
         preempt(topo, free, pods, lvl, hold, W, mem=None, base=0) -> (keys, victims)):
-    tests/gang_twin/gang_twin.c and tests/preempt_twin/preempt_twin.c built with the oracle into a temporary directory."""
-    d = tmp_path_factory.mktemp("weight_twins")
-    libs = {}
-    for name, src in (("gang", os.path.join(HERE, "gang_twin", "gang_twin.c")), ("preempt", os.path.join(HERE, "preempt_twin", "preempt_twin.c"))):
-        so = str(d / ("lib%s_twin.so" % name))
-        subprocess.check_call(["gcc", "-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11", "-pthread", "-shared", "-o", so,
-                               os.path.join(ROOT, "oracle", "oracle_b.c"), src])
-        libs[name] = ctypes.CDLL(so)
-    G, Pr = libs["gang"], libs["preempt"]
-    G.gang_twin_place_batch.restype = None
-    G.gang_twin_place_batch.argtypes = [_i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p, ctypes.c_int64, _i32p, _u64p]
-    Pr.preempt_twin_batch.restype = None
-    Pr.preempt_twin_batch.argtypes = [_i32p, _i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p, ctypes.c_int64,
-                                      _i32p, ctypes.c_int, _u64p, _u32p]
+    tests/gang_twin/gang_twin.c and tests/preempt_twin/preempt_twin.c built with the oracle."""
+    G, Pr = cpu_libs.twin("gang"), cpu_libs.twin("preempt")
 
     def gang(topo, free, pods, gang, W, mem=None, base=0):
         topo, pods, gang, W = (np.ascontiguousarray(a, dtype=np.int32) for a in (topo, pods, gang, W))
@@ -363,29 +348,9 @@ def test_zero_table_is_the_tie_break(oracle_b):
 
 # ---- CPU: the kernel sources (tests/emu) against the twins ---------------------------------------------------------------
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    """The scoring and placement kernels (tests/emu), the gang kernel and the preemption kernels, each built for the CPU."""
-    subprocess.check_call(["make", "-s", "-C", os.path.join(HERE, "emu")])
-    L = ctypes.CDLL(os.path.join(HERE, "emu", "_build", "libkgpu_emu.so"))
-    for fn in (L.emu_score_sparse, L.emu_score_dense):
-        fn.restype = None
-        fn.argtypes = [_i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, ctypes.c_int64, _i32p, ctypes.c_int, _u64p]
-    L.emu_score_variant.restype = None
-    L.emu_score_pair_list.restype = None
-    L.emu_fit_nodes.restype = None
-    L.emu_place_batch.restype = ctypes.c_int
-    d = tmp_path_factory.mktemp("weight_emu")
-    for name, src in (("gang", os.path.join(HERE, "gang_twin", "emu_gang.cc")), ("preempt", os.path.join(HERE, "preempt_twin", "emu_preempt.cc"))):
-        so = str(d / ("lib%s_emu.so" % name))
-        subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I" + os.path.join(HERE, "emu", "stub"),
-                               "-I" + os.path.join(HERE, "emu"), "-I" + os.path.join(ROOT, "kubegpu_b200", "csrc"), "-o", so, src])
-        setattr(L, name, ctypes.CDLL(so))
-    L.gang.emu_place_batch_gang.restype = ctypes.c_int
-    L.gang.emu_place_batch_gang.argtypes = [_i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p, ctypes.c_int64, _i32p, _u64p]
-    L.preempt.emu_preempt_batch.restype = ctypes.c_int
-    L.preempt.emu_preempt_batch.argtypes = [_i32p, _i32p, _i32p, _i32p, ctypes.c_int64, ctypes.c_int64, _i32p, _i32p, ctypes.c_int64,
-                                            _i32p, ctypes.c_int, _u64p, _u32p]
-    return L
+def emu():
+    """The kernels compiled for the CPU (tests/emu)."""
+    return cpu_libs.emu()
 
 
 def emu_score(fn, topo, free, pods, W, mem=None, base=0, splits=1):
@@ -526,7 +491,7 @@ def emu_gang(emu, topo, free, pods, gang, W, mem=None, base=0):
     f = np.array(free, dtype=np.int32, copy=True)
     topo, pods, gang, W = (np.ascontiguousarray(a, dtype=np.int32) for a in (topo, pods, gang, W))
     keys = np.empty(len(pods), dtype=np.uint64)
-    assert emu.gang.emu_place_batch_gang(_p(topo), _p(f), _opt(mem), len(f), base, _p(pods), _p(gang), len(pods), _p(W),
+    assert emu.emu_place_batch_gang(_p(topo), _p(f), _opt(mem), len(f), base, _p(pods), _p(gang), len(pods), _p(W),
                                          _p(keys, ctypes.c_uint64)) == 0
     return keys, f
 
@@ -552,7 +517,7 @@ def emu_preempt(emu, oracle_b, topo, free, pods, lvl, hold, W, mem=None, base=0,
     topo, free, pods, lvl, W = (np.ascontiguousarray(a, dtype=np.int32) for a in (topo, free, pods, lvl, W))
     keys = oracle_b.score_batch(topo, free, pods, W, mem=mem, node_id_base=base)
     vic = np.empty(len(pods), dtype=np.uint32)
-    reached = emu.preempt.emu_preempt_batch(_p(topo), _p(free), _opt(mem), _opt(hold), len(free), base, _p(pods), _p(lvl), len(pods),
+    reached = emu.emu_preempt_batch(_p(topo), _p(free), _opt(mem), _opt(hold), len(free), base, _p(pods), _p(lvl), len(pods),
                                             _p(W), splits, _p(keys, ctypes.c_uint64), _p(vic, ctypes.c_uint32))
     return keys, vic, reached
 
