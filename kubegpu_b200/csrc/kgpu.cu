@@ -48,7 +48,7 @@ struct kgpu_shard {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     kgpu::DeviceBuffer<int32_t> d_topo;   // [n][64]
     kgpu::DeviceBuffer<int32_t> d_free;   // [n]
-    kgpu::DeviceBuffer<int32_t> d_mem;    // [n][8] MiB per GPU (0x7F7F7F7F = unconstrained until uploaded)
+    kgpu::DeviceBuffer<int32_t> d_mem;    // [n][8] MiB per GPU (INT32_MAX = unconstrained until uploaded)
     kgpu::DeviceBuffer<int> d_flag;       // "batch has memory-constrained pods"
     kgpu::DeviceBuffer<int4> d_rec;       // K1s: [tiles][7][SP_THREADS] compacted scaled pair costs, slot order (compact_nodes)
     kgpu::DeviceBuffer<uint32_t> d_meta;  // K1s: [n_slots] position -> GPU index (3-bit fields) | free count << 24
@@ -596,8 +596,9 @@ int upload_nodes(kgpu_ctx *h, const int32_t *topo, const int32_t *free_mask, int
         KGPU_CUDA(h, s.d_mem.reserve(8 * cnt));
         KGPU_CUDA(h, s.d_slot_of.reserve(cnt));
         if (cnt > 0) {
-            // per-GPU memory is unconstrained (0x7F7F7F7F MiB) until kgpu_upload_gpu_memory says otherwise
-            KGPU_CUDA(h, cudaMemsetAsync(s.d_mem, 0x7F, (size_t)cnt * 32, s.stream));
+            // per-GPU memory is unconstrained (INT32_MAX MiB) until kgpu_upload_gpu_memory says otherwise
+            kgpu::fill_i32<<<(unsigned)((cnt * 8 + 255) / 256), 256, 0, s.stream>>>(s.d_mem, cnt * 8, INT32_MAX);
+            h->launches++;
             KGPU_CUDA(h, cudaMemcpyAsync(s.d_topo, topo + off * 64, (size_t)cnt * 256, cudaMemcpyHostToDevice, s.stream));
             KGPU_CUDA(h, cudaMemcpyAsync(s.d_free, free_mask + off, (size_t)cnt * 4, cudaMemcpyHostToDevice, s.stream));
             // value-domain check on the device (levels 0..15): one 8-byte read-back instead of an O(64 N) host pass

@@ -117,6 +117,13 @@ order_scatter(const int32_t *__restrict__ free_mask, int64_t N, const int32_t *_
     slot_of[node] = slot;
 }
 
+// p[0..n) = v.  kgpu_upload_nodes: every GPU's memory is INT32_MAX MiB until kgpu_upload_gpu_memory, so that no positive
+// min_mem excludes it (a byte-wise memset reaches only 0x7F7F7F7F, which a requirement above it would fail).
+__global__ void fill_i32(int32_t *__restrict__ p, int64_t n, int32_t v) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) p[i] = v;
+}
+
 __global__ void scatter_masks(const int32_t *__restrict__ idx, const int32_t *__restrict__ mask, int64_t n, int32_t *free_mask) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) free_mask[idx[i]] = mask[i];

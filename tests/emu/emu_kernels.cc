@@ -54,8 +54,12 @@ struct Staging {
     }
     int4 *topo(const int32_t *topo, int64_t n) { return copy<int4>(topo, (size_t)n * 16); }
     int4 *pods(const int32_t *pods, int64_t P) { return copy<int4>(pods, (size_t)P); }
-    // GPU memory per node: unconstrained (0x7F7F7F7F MiB) without an upload, as in kgpu.cu
-    int32_t *mem(const int32_t *gpu_mem, int64_t n) { return copy<int32_t>(gpu_mem, (size_t)n * 8, 0x7F); }
+    // GPU memory per node: unconstrained (INT32_MAX MiB) without an upload, as in kgpu.cu
+    int32_t *mem(const int32_t *gpu_mem, int64_t n) {
+        int32_t *p = copy<int32_t>(gpu_mem, (size_t)n * 8);
+        if (!gpu_mem) std::fill(p, p + n * 8, INT32_MAX);
+        return p;
+    }
 };
 
 void upload_subset_tables() { kgpu::subset_tables(kgpu::c_subsets, kgpu::c_nsub); }
