@@ -25,6 +25,9 @@ EMU_SIGNATURES = {
     "emu_score_dense": (None, _SCORE),
     "emu_score_variant": (None, [_int] + _SCORE),
     "emu_score_sparse_after_updates": (None, [_i32p, _i32p, _i64, _i32p, _i32p, _i64, _i32p, _i64, _i32p, _int, _u64p, _i32p]),
+    # topo0, free0, mem, n, base, upd_idx, upd_mask, upd_topo, has_topo, m, W, W2, w2_at, pods, P, splits, keys, free_out
+    "emu_score_sparse_sequence": (_int, [_i32p, _i32p, _i32p, _i64, _i64, _i32p, _i32p, _i32p, _i32p, _i64, _i32p, _i32p, _i64,
+                                         _i32p, _i64, _int, _u64p, _i32p]),
     "emu_order": (_i64, [_i32p, _i64, _i32p, _i64, _i32p, _i64p]),
     "emu_tile_classes": (_i64, [_i32p, _i64, _int, _u8p, _u8p, _i64]),
     "emu_fit_nodes": (None, [_i32p, _i32p, _i64, _i32p, _i64, _i32p, _u32p]),

@@ -192,6 +192,67 @@ void emu_score_sparse_after_updates(const int32_t *topo, const int32_t *free_mas
     std::memcpy(free_mask_out, free_mask.data(), (size_t)n * 4);
 }
 
+// A handle's K1s cache over a sequence of state changes, then K1s.  The cache is built for (topo0, free0) as by
+// kgpu_upload_nodes; update j then goes through the incremental path on the order that stays as it was (stale):
+//   has_topo[j] == 0  kgpu_set_free_masks: consecutive such updates are one batched compact_nodes(list, new_mask), a batch
+//                     being cut where a node repeats;
+//   has_topo[j] != 0  kgpu_update_node: row j of upd_topo is written over the node's topology, then compact_nodes over
+//                     that one node with its new mask.
+// With W2, before update w2_at (after the last one if w2_at >= m) the weights become W2 the way kgpu_set_weights +
+// ensure_node_cache apply them: one compact_nodes over every slot of the stale order, no re-sort; later updates use W2.
+// K1s then runs with the final weights (route and splits as for emu_score_sparse, which it returns the route code of);
+// free_out receives the final masks.
+int emu_score_sparse_sequence(const int32_t *topo0, const int32_t *free0, const int32_t *gpu_mem /*nullable*/, int64_t n,
+                              int64_t node_id_base, const int32_t *upd_idx, const int32_t *upd_mask, const int32_t *upd_topo,
+                              const int32_t *has_topo, int64_t m, const int32_t *W, const int32_t *W2 /*nullable*/, int64_t w2_at,
+                              const int32_t *pods, int64_t P, int splits, unsigned long long *keys, int32_t *free_out) {
+    std::memset(keys, 0xFF, (size_t)P * 8);
+    if (n == 0 || P == 0) return -1;
+    std::vector<int32_t> free_mask(free0, free0 + n);
+    Staging st;
+    int4 *topo4 = st.topo(topo0, n);
+    kgpu::Weights Ws = weights_of(W);
+    const int32_t *Wcur = W;
+    Cache c(free_mask.data(), n, 32, topo4, &Ws);
+    std::vector<int32_t> bidx, bmask;
+    auto refresh = [&](const int32_t *idx, const int32_t *mask, int64_t cnt) {
+        emu::launch(dim3((unsigned)((cnt + kgpu::SP_THREADS - 1) / kgpu::SP_THREADS)), dim3(kgpu::SP_THREADS), [&] {
+            kgpu::compact_nodes(topo4, free_mask.data(), cnt, Ws, c.order.data(), c.slot_of.data(), c.rec, c.meta, idx, mask);
+        });
+    };
+    auto flush = [&] {
+        if (!bidx.empty()) refresh(bidx.data(), bmask.data(), (int64_t)bidx.size());
+        bidx.clear();
+        bmask.clear();
+    };
+    auto set_weights = [&] {
+        flush();
+        Ws = weights_of(W2);
+        Wcur = W2;
+        emu::launch(dim3((unsigned)(c.n_slots / kgpu::SP_THREADS)), dim3(kgpu::SP_THREADS), [&] {
+            kgpu::compact_nodes(topo4, free_mask.data(), c.n_slots, Ws, c.order.data(), c.slot_of.data(), c.rec, c.meta);
+        });
+    };
+    for (int64_t j = 0; j < m; j++) {
+        if (W2 && j == w2_at) set_weights();
+        if (has_topo[j]) {
+            flush();
+            std::memcpy(reinterpret_cast<int32_t *>(topo4) + (int64_t)upd_idx[j] * 64, upd_topo + j * 64, 256);
+            refresh(upd_idx + j, upd_mask + j, 1);
+        } else {
+            if (std::find(bidx.begin(), bidx.end(), upd_idx[j]) != bidx.end()) flush();
+            bidx.push_back(upd_idx[j]);
+            bmask.push_back(upd_mask[j]);
+        }
+    }
+    if (W2 && w2_at >= m) set_weights();
+    flush();
+    const K1sRun run = launch_k1s(c, st.mem(gpu_mem, n), node_id_base, st.pods(pods, P), P, Wcur, splits, true, keys);
+    std::memcpy(free_out, free_mask.data(), (size_t)n * 4);
+    const kgpu::SparseRoute &r = run.route;
+    return (r.tma ? 3 : r.stream ? 2 : r.prepared ? 1 : 0) | (run.mem ? 4 : 0) | (r.byte_keys ? 8 : 0);
+}
+
 // The device-built order alone: order[cap] (cap = n + 9*32 + 2*tile rounded down to tiles), slot_of[n], class counts.
 int64_t emu_order(const int32_t *free_mask, int64_t n, int32_t *order_out, int64_t cap, int32_t *slot_of_out, long long *class_count) {
     std::vector<int32_t> f(free_mask, free_mask + n);

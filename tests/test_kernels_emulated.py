@@ -413,3 +413,92 @@ def test_emulated_k1s_routes(emu, oracle_b, route, mem, byte_keys):
     got = emu.emu_score_sparse(_p(topo), _p(free), _p(gmem), len(free), 5, _p(pods), P, _p(W), splits, _p(keys, ctypes.c_uint64))
     assert got == K1S_ROUTES[route] | (4 if mem else 0) | (8 if byte_keys else 0)
     assert (keys == want).all()
+
+
+# ---- a handle's K1s cache over a sequence of state changes, on every route -----------------------------------------
+ALL_FIFTEEN = np.full(64, 15, dtype=np.int32)          # every link on level 15: the cheapest level of the tables below
+
+
+def _order_layout(emu, free):
+    """The order kgpu_upload_nodes builds for these masks: order[n_slots] (-1 = padding) and its 128-slot tiles."""
+    n = len(free)
+    cap = (n + 11 * 128) // 128 * 128
+    order, slot_of, cc = np.empty(cap, np.int32), np.empty(n, np.int32), np.empty(9, np.int64)
+    n_slots = emu.emu_order(_p(free), n, _p(order), cap, _p(slot_of), _p(cc, ctypes.c_longlong))
+    return order[:n_slots], slot_of
+
+
+def _sequence_updates(emu, topo, free):
+    """(updates, named nodes): a list of (node, new mask, new topology row or None) that covers a node going from 0 to 8
+    free GPUs and one from 8 to 0, a node changing class in an ordered tile (one class, ids increasing) and one in a
+    mixed-class tile, the last node, the node just before a run of padding slots, a node updated twice, node A made the
+    unique cheapest node by its topology and node B, with a lower id in another tile, tied with A for k <= 4."""
+    order, slot_of = _order_layout(emu, free)
+    pop = np.array([bin(int(f) & 0xFF).count("1") for f in free])
+    tiles = order.reshape(-1, 128)
+    ordered = [t for t in range(len(tiles))
+               if all(tiles[t][i] < 0 or (tiles[t][i - 1] >= 0 and tiles[t][i - 1] < tiles[t][i]) for i in range(1, 128))]
+    mixed = [t for t in range(len(tiles)) if len({int(pop[x]) for x in tiles[t] if x >= 0}) > 1]
+    assert ordered and mixed
+    in_ordered = int(tiles[ordered[0]][5])
+    in_mixed = next(int(x) for x in tiles[mixed[0]] if x >= 0 and pop[x] not in (0, 8))
+    before_pad = next(int(order[s]) for s in range(len(order) - 1) if order[s] >= 0 and order[s + 1] < 0)
+    empty = next(i for i in range(len(free)) if pop[i] == 0 and i not in (in_ordered, in_mixed, before_pad))
+    full = next(i for i in range(len(free)) if pop[i] == 8 and i not in (in_ordered, in_mixed, before_pad))
+    a = len(free) - 40
+    b = next(i for i in range(len(free) // 3) if slot_of[i] // 128 != slot_of[a] // 128 and
+             i not in (in_ordered, in_mixed, before_pad, empty, full))
+    named = dict(a=a, b=b, in_ordered=in_ordered, in_mixed=in_mixed, before_pad=before_pad, empty=empty, full=full,
+                 last=len(free) - 1)
+    upd =[(empty, 0xFF, None), (full, 0x00, None),
+           (in_ordered, 0xFF if pop[in_ordered] < 8 else 0x01, None), (in_mixed, 0x80 if pop[in_mixed] > 1 else 0xFE, None),
+           (a, 0xFF, ALL_FIFTEEN), (len(free) - 1, 0xF7, None), (before_pad, 0x3C, None),
+           (in_mixed, 0xFF, None), (b, 0x0F, ALL_FIFTEEN), (len(free) - 1, 0xFF, topo[0].copy()),
+           (before_pad, 0xFF, topo[1].copy())]
+    return upd, named
+
+
+@pytest.mark.parametrize("route", sorted(K1S_ROUTES))
+@pytest.mark.parametrize("mem", [False, True])
+@pytest.mark.parametrize("byte_keys", [True, False])
+def test_emulated_k1s_after_a_sequence_of_state_changes(emu, oracle_b, route, mem, byte_keys):
+    """K1s on records refreshed in place while the order stays stale (kgpu_set_free_masks, kgpu_update_node with a new
+    topology) and recompacted over the stale order by a weight change half way through, on each route, with and without
+    the MEM launch, byte and general keys, a node-id base and GPU memory: Oracle B's keys on the final state."""
+    P, splits = {"tma": (40, -1), "stream": (300, -1), "prepared": (600, -1), "in_block_sort": (600, -1184)}[route]
+    N, base = 700, 1000
+    topo, free, _ = synth.gen_c2(N=N, P=0, seed=77)            # four shapes: cost ties across nodes and tiles are the rule
+    topo, free = topo.copy(), free.copy()
+    gmem = synth.gen_gpu_memory(N, seed=78)
+    _, _, _, pods = synth.gen_c6(N=1, P=P, seed=P)
+    pods[2, 0], pods[3, 0] = 0, 9
+    if not mem:
+        pods[:, 3] = 0
+    top = 2340 if byte_keys else 2341
+    W = np.array([top - 5 * i for i in range(16)], dtype=np.int32)
+    W2 = W.copy()
+    W2[1], W2[5] = W[5], W[1]                                   # C2's levels 1 and 5 swap costs; level 15 stays cheapest
+    upd, named = _sequence_updates(emu, topo, free)
+    gmem[[named["a"], named["b"]]] = synth.GPU_MEM_CLASSES_MIB[-1]
+    m = len(upd)
+    idx = np.array([u[0] for u in upd], np.int32)
+    masks = np.array([u[1] for u in upd], np.int32)
+    rows = np.stack([u[2] if u[2] is not None else np.zeros(64, np.int32) for u in upd]).astype(np.int32)
+    has = np.array([u[2] is not None for u in upd], np.int32)
+    final_topo, final_free = topo.copy(), free.copy()
+    for i, mk, row in upd:
+        final_free[i] = mk
+        if row is not None:
+            final_topo[i] = row
+    want = oracle_b.score_batch(final_topo, final_free, pods, W2, node_id_base=base, mem=gmem, fast=True, nthreads=4)
+    winners = {int(k >> np.uint64(8)) & 0xFFFFFFFF for k in want if k != np.uint64(0xFFFFFFFFFFFFFFFF)}
+    assert {named["a"] + base, named["b"] + base} <= winners          # A wins k > 4, B (lower id, another tile) k <= 4
+    keys = np.empty(P, np.uint64)
+    out_free = np.empty(N, np.int32)
+    got = emu.emu_score_sparse_sequence(_p(topo), _p(free), _p(gmem), N, base, _p(idx), _p(masks), _p(rows), _p(has), m,
+                                        _p(W), _p(W2), m // 2, _p(pods), P, splits, _p(keys, ctypes.c_uint64), _p(out_free))
+    assert got == K1S_ROUTES[route] | (4 if mem else 0) | (8 if byte_keys else 0)
+    assert (out_free == final_free).all()
+    bad = np.flatnonzero(keys != want)
+    assert len(bad) == 0, "%d keys differ, first pod %d (k %d): got %x want %x" % (
+        len(bad), bad[0], pods[bad[0], 0], int(keys[bad[0]]), int(want[bad[0]]))
