@@ -133,6 +133,44 @@ func (k *handle) placeBatch(pods []int32, gang []int32, dryRun bool) ([]uint64, 
 	return keys, nil
 }
 
+// uploadDomains: each node's network domain, -1 (none) or 0..n-1 (kgpu_upload_domains); len(domain) = the node count.
+func (k *handle) uploadDomains(domain []int32) error {
+	var d *C.int32_t
+	if len(domain) > 0 {
+		d = (*C.int32_t)(unsafe.Pointer(&domain[0]))
+	}
+	if rc := C.kgpu_upload_domains(k.h, d, C.int64_t(len(domain))); rc != C.KGPU_OK {
+		return k.err("kgpu_upload_domains")
+	}
+	return nil
+}
+
+// placeBatchDomain: placeBatch with one gang_domain value per pod (kgpu_place_batch_gang_domain): 0 = no constraint,
+// C.KGPU_GANG_DOMAIN_REQUIRED = the gang inside one domain or not at all, C.KGPU_GANG_DOMAIN_PREFERRED = inside one
+// domain if one fits, else as a plain gang.  gangDomain nil is placeBatch.
+func (k *handle) placeBatchDomain(pods []int32, gang []int32, gangDomain []int32, dryRun bool) ([]uint64, error) {
+	keys := make([]uint64, len(pods)/4)
+	if len(keys) == 0 {
+		return keys, nil
+	}
+	flags := C.int(0)
+	if dryRun {
+		flags = C.KGPU_PLACE_DRY_RUN
+	}
+	var g, gd *C.int32_t
+	if gang != nil {
+		g = (*C.int32_t)(unsafe.Pointer(&gang[0]))
+	}
+	if gangDomain != nil {
+		gd = (*C.int32_t)(unsafe.Pointer(&gangDomain[0]))
+	}
+	if rc := C.kgpu_place_batch_gang_domain(k.h, (*C.int32_t)(unsafe.Pointer(&pods[0])), g, gd, C.int64_t(len(keys)),
+		(*C.uint64_t)(unsafe.Pointer(&keys[0])), flags); rc != C.KGPU_OK {
+		return nil, k.err("kgpu_place_batch_gang_domain")
+	}
+	return keys, nil
+}
+
 func (k *handle) freeMasks(n int64) ([]int32, error) {
 	out := make([]int32, n)
 	if n == 0 {

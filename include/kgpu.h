@@ -20,7 +20,7 @@
  *          batched over every (pod, node) pair instead of one cgo call per pair
  *   kgpu_fit_lookup / kgpu_build_fit_table / kgpu_score_pairs
  *       <- the same PodFitsDevice, called once per (node, pod) by the core: served from a host-side (node, k) table
- *   kgpu_set_free_mask[s] / kgpu_place_batch[_ex|_gang] / kgpu_get_free_masks
+ *   kgpu_set_free_mask[s] / kgpu_place_batch[_ex|_gang|_gang_domain] / kgpu_upload_domains / kgpu_get_free_masks
  *       <- TakePodResources / ReturnPodResources       gpuschedulerplugin/gpu_scheduler.go:57-63 (no-ops there)
  *   kgpu_reduce_shards_device
  *       <- (no reference counterpart; the reference is single-process) the final
@@ -195,6 +195,41 @@ int kgpu_place_batch_ex(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out
  * kgpu_place_batch_ex on the batch with every failed gang deleted.  Members may differ in k and min_mem_mib.
  * gang == NULL is kgpu_place_batch_ex.  Flags, min_mem_mib limits and single-device handles as there. */
 int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, int64_t P, uint64_t *out_keys, int flags);
+/* Gangs inside one network domain.  For a multi-node job the inter-node network carries the all-reduce, so where the
+ * members sit relative to each other matters as much as the GPUs inside each node.
+ *
+ * Each node has a DOMAIN: -1 (none) or an id 0 <= d < n (n = kgpu_num_nodes).  A domain is the set of nodes under one
+ * leaf switch, one InfiniBand scalable unit or one NVLink Switch domain; the caller decides.  kgpu_upload_domains sets
+ * the whole table (n entries; a value outside -1..n-1 is KGPU_ERR_INVALID and leaves the table unchanged).  Until the
+ * first upload every node's domain is -1; kgpu_upload_nodes resets the table to all -1, and kgpu_update_node,
+ * kgpu_set_free_mask(s) and kgpu_remove_node leave it alone.  Scoring ignores domains, so an upload invalidates nothing.
+ *
+ * Each pod has a gang_domain value: 0 (no constraint), KGPU_GANG_DOMAIN_REQUIRED or KGPU_GANG_DOMAIN_PREFERRED.  Pods
+ * are taken in order on the working masks F exactly as by kgpu_place_batch_gang, and pods and gangs with gang_domain 0
+ * are placed exactly as there.  A CONSTRAINED gang has members m1..mj, consecutive pods with the same nonzero gang id,
+ * all carrying the same nonzero gang_domain.  It is placed like this:
+ *   1. Trial per domain.  For every domain d with at least one node, a trial on a copy F_d of F: for i = 1..j, if
+ *      k(m_i) is outside 0..8 the trial fails; otherwise key_i = the minimum of (cost << 40 | node_id << 8 | S) over
+ *      the nodes n with domain[n] = d, under F_d, with m_i's min_mem_mib applied as in scoring; if key_i is KGPU_NO_FIT
+ *      the trial fails, otherwise F_d[n] &= ~S.  A trial that places every member has C_d = the sum of the members'
+ *      costs.  A k = 0 member costs 0, takes nothing and gets the domain's lowest node.
+ *   2. Choice.  If some trial succeeded, the gang takes the domain d* with the smallest (C_d, d): F = F_d*, and the
+ *      members get that trial's keys.
+ *   3. No domain fits, REQUIRED: every member gets KGPU_NO_FIT, and F is unchanged.
+ *   4. No domain fits, PREFERRED: the gang is placed exactly as kgpu_place_batch_gang would place it on F: over all
+ *      nodes, all or nothing.
+ * So gang_domain == NULL (or all 0) is kgpu_place_batch_gang; with every node in domain 0, REQUIRED and PREFERRED both
+ * are kgpu_place_batch_gang; the members of a placed REQUIRED gang sit in one domain, never on a node of domain -1; and a
+ * PREFERRED gang gets the REQUIRED result when some domain fits, the plain gang result otherwise.
+ * KGPU_ERR_INVALID, checked before anything runs: a gang_domain value outside {0, 1, 2}, a nonzero value on a pod with
+ * gang id 0, members of one gang that disagree, a constrained gang of more than 37 000 members (the trials sum their
+ * costs in 32 bits), and the checks of kgpu_place_batch_gang.  Flags (KGPU_PLACE_DRY_RUN) as there.  Both calls need
+ * a single-device handle (KGPU_ERR_STATE otherwise).  Host buffers, synchronous. */
+#define KGPU_GANG_DOMAIN_REQUIRED 1
+#define KGPU_GANG_DOMAIN_PREFERRED 2
+int kgpu_upload_domains(kgpu_t *h, const int32_t *domain, int64_t n);
+int kgpu_place_batch_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *gang, const int32_t *gang_domain,
+                                 int64_t P, uint64_t *out_keys, int flags);
 /* Preemption (kube-scheduler's PostFilter for GPU pods): for a pod that fits nowhere, the node, GPUs and
  * lowest-priority running pods to evict.  No reference counterpart (DeviceScheduler has no preemption hook,
  * gpu_scheduler.go:21-71).  Single-device handles only (KGPU_ERR_STATE otherwise).

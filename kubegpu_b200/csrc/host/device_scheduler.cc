@@ -83,6 +83,7 @@ using gpuplugintypes::ResourceGPU;
 const char *const GPUTopologyGeneration = "gpu/gpu-generate-topology";
 const char *const GPUMinMemoryMiB = "gpu/gpu-min-memory-mib";
 const char *const GPUGangID = "gpu/gpu-gang-id";
+const char *const GPUGangDomain = "gpu/gpu-gang-domain";
 const char *const GPUPriorityLevel = "gpu/gpu-priority-level";
 
 namespace {
@@ -506,6 +507,33 @@ std::string NvidiaGPUScheduler::AddNodeFromGpusInfo(const std::string &nodeName,
     return SetNodeTopology(nodeName, topo);
 }
 
+std::string NvidiaGPUScheduler::SetNodeDomain(const std::string &nodeName, const std::string &domainName) {
+    auto it = nodes_.find(nodeName);
+    if (it == nodes_.end()) return lastError_ = "SetNodeDomain: unknown node " + nodeName;
+    if (it->second.domain != domainName) domainsDirty_ = true;
+    it->second.domain = domainName;
+    return "";
+}
+
+// The domain table on the device, if a domain or the node array changed since the last push: names -> ids 0, 1, ... in
+// sorted order, -1 for nodes without one.
+std::string NvidiaGPUScheduler::pushDomains() {
+    if (!domainsDirty_) return "";
+    std::map<std::string, int32_t> ids;
+    for (const std::string &name : indexToName_)
+        if (!nodes_[name].domain.empty()) ids.emplace(nodes_[name].domain, 0);
+    int32_t next = 0;
+    for (auto &kv : ids) kv.second = next++;
+    std::vector<int32_t> domain(indexToName_.size(), -1);
+    for (size_t i = 0; i < indexToName_.size(); i++) {
+        const std::string &d = nodes_[indexToName_[i]].domain;
+        if (!d.empty()) domain[i] = ids[d];
+    }
+    if (kgpu_upload_domains(handle_, domain.data(), (int64_t)domain.size()) != KGPU_OK) return lastError_ = kgpu_last_error(handle_);
+    domainsDirty_ = false;
+    return "";
+}
+
 // Push the host-side node array to the device(s) if it changed since the last launch.
 std::string NvidiaGPUScheduler::flushNodes() {
     if (!handle_) return lastError_ = "no CUDA device: the kgpu scorer has no CPU path (" + lastError_ + ")";
@@ -546,6 +574,7 @@ std::string NvidiaGPUScheduler::flushNodes() {
     if (anyMem && kgpu_upload_gpu_memory(handle_, mem.data(), (int64_t)n) != KGPU_OK) return lastError_ = kgpu_last_error(handle_);
     dirty_ = false;
     holdersReset_ = true;                                // kgpu_upload_nodes reset the holder table
+    domainsDirty_ = true;                                // and the domain table
     return "";
 }
 
@@ -637,9 +666,24 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     // ids are renumbered 1, 2, ... in order of first appearance (no truncation can merge two gangs) and each member
     // moves up to its gang's first member.  order[i] = the caller's index of the pod at device position i.
     std::vector<size_t> order(P);
-    std::vector<int32_t> gang;
+    std::vector<int32_t> gang, gangDomain;          // gangDomain: in device order, empty when no pod asks for a domain
     for (size_t p = 0; p < P; p++) order[p] = p;
-    if (mode == BatchMode::Sequential || mode == BatchMode::DryRun || mode == BatchMode::PreemptGangPlan) {
+    const bool placing = mode == BatchMode::Sequential || mode == BatchMode::DryRun;
+    if (placing) {
+        std::map<int64_t, int64_t> domainOfGang;
+        for (size_t p = 0; p < P; p++) {
+            const int64_t gd = getOr0(pods[p]->Requests, GPUGangDomain), id = getOr0(pods[p]->Requests, GPUGangID);
+            if (gd != 0 && gd != KGPU_GANG_DOMAIN_REQUIRED && gd != KGPU_GANG_DOMAIN_PREFERRED)
+                return lastError_ = "pod " + pods[p]->Name + ": " + GPUGangDomain + " must be 1 (required) or 2 (preferred)";
+            if (gd != 0 && id == 0) return lastError_ = "pod " + pods[p]->Name + ": " + GPUGangDomain + " without " + GPUGangID;
+            if (id != 0 && !domainOfGang.emplace(id, gd).second && domainOfGang[id] != gd)
+                return lastError_ = "pod " + pods[p]->Name + ": the members of gang " + std::to_string(id) + " disagree on " + GPUGangDomain;
+            if (gd != 0) gangDomain.assign(P, 0);
+        }
+        err = pushDomains();
+        if (!err.empty()) return err;
+    }
+    if (placing || mode == BatchMode::PreemptGangPlan) {
         std::map<int64_t, int32_t> dense;
         std::vector<std::vector<size_t>> members;
         std::vector<int32_t> gangOf(P, 0);
@@ -673,6 +717,7 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     std::vector<int32_t> req(P * 4, 0);
     for (size_t i = 0; i < P; i++) {
         const size_t p = order[i];
+        if (!gangDomain.empty()) gangDomain[i] = (int32_t)getOr0(pods[p]->Requests, GPUGangDomain);
         types::PodInfo copy = *pods[p];                    // SetGPUReqs mutates; keep the caller's pod intact
         for (auto &c : copy.InitContainers) SetGPUReqs(c.second);
         for (auto &c : copy.RunningContainers) SetGPUReqs(c.second);
@@ -696,9 +741,9 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
                        ? kgpu_preempt_plan_gang(handle_, req.data(), lvl.data(), gang.empty() ? nullptr : gang.data(), (int64_t)P,
                                                 dev.data(), owners.data())
                    : mode == BatchMode::Snapshot ? kgpu_score_batch(handle_, req.data(), (int64_t)P, dev.data())
-                                               : kgpu_place_batch_gang(handle_, req.data(), gang.empty() ? nullptr : gang.data(),
-                                                                       (int64_t)P, dev.data(),
-                                                                       mode == BatchMode::DryRun ? KGPU_PLACE_DRY_RUN : 0);
+                                               : kgpu_place_batch_gang_domain(handle_, req.data(), gang.empty() ? nullptr : gang.data(),
+                                                                              gangDomain.empty() ? nullptr : gangDomain.data(), (int64_t)P,
+                                                                              dev.data(), mode == BatchMode::DryRun ? KGPU_PLACE_DRY_RUN : 0);
     if (rc != KGPU_OK) return lastError_ = kgpu_last_error(handle_);
     std::vector<uint64_t> keys(P, KGPU_NO_FIT);           // back in the caller's order
     std::vector<uint32_t> vic(P, 0);

@@ -93,6 +93,11 @@ extern const char *const GPUMinMemoryMiB;         // "gpu/gpu-min-memory-mib"
 // distributed training job).  Pods of one PlaceBatch / ProposeBatch call with the same nonzero value are placed all
 // or nothing; 0 or absent = the pod is on its own.
 extern const char *const GPUGangID;               // "gpu/gpu-gang-id"
+// Extension: pod-level request "my gang wants one network domain" (SetNodeDomain): 1 = required (the gang is placed
+// inside one domain or not at all), 2 = preferred (inside one domain if one fits, else as a plain gang), 0 or absent =
+// no constraint.  Only on gang members, the same for every member of a gang; honoured by PlaceBatch and ProposeBatch
+// (kgpu_place_batch_gang_domain).
+extern const char *const GPUGangDomain;           // "gpu/gpu-gang-domain"
 // Extension: pod-level request "my priority level", 0..15 (values outside are clamped), default 0.  PreemptBatch lets a
 // pod evict running pods of a LOWER level; every placement records the level of its pod.
 extern const char *const GPUPriorityLevel;        // "gpu/gpu-priority-level"
@@ -174,20 +179,26 @@ public:
     // Real NVML link matrix for a node (int32[8][8] row-major, levels 0..15) instead of the
     // one derived from its 2-level group names.
     std::string SetNodeTopology(const std::string &nodeName, const int32_t topo[64]);
+    // The network domain of a node (the nodes under one leaf switch, one scalable unit or one NVLink Switch domain);
+    // "" = none, the default.  Names map to dense ids in sorted order; the device table is re-uploaded before the next
+    // PlaceBatch / ProposeBatch when a domain or the node array has changed.
+    std::string SetNodeDomain(const std::string &nodeName, const std::string &domainName);
     // Node from the node agent's GPU inventory JSON (nvgputypes.GpusInfo): names exactly as the
     // agent would advertise them, then AddNode, then the REAL link matrix (not the one implied by
     // the two group levels).  Fills *nodeInfo like the agent's UpdateNodeInfo.  "" or error text.
     std::string AddNodeFromGpusInfo(const std::string &nodeName, const std::string &gpusInfoJSON, bool useNVML,
                                     types::NodeInfo *nodeInfo);
-    // Score a whole scheduling cycle in one kernel launch: best node + GPU set per pod.  Gang ids are ignored:
-    // snapshot scores change no state, so there is nothing to keep all or nothing.
+    // Score a whole scheduling cycle in one kernel launch: best node + GPU set per pod.  Gang ids and gang domains are
+    // ignored: snapshot scores change no state, so there is nothing to keep all or nothing or together.
     std::string ScoreBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out);
     // Place a whole cycle IN ORDER on the device: each pod takes its GPUs before the next one is
     // scored (K3).  The placements are remembered like ScoreBatch's and the usage is recorded, so a
     // later PodAllocate / ReturnPodResources works on them.  Gangs (GPUGangID): every member is placed right after
     // the gang's first member in the batch (the others keep their order); if one member does not fit, the whole gang
-    // gets fits = false, takes nothing, and the pods after it are placed as if it had not been in the batch.  `out`
-    // is in the caller's order.
+    // gets fits = false, takes nothing, and the pods after it are placed as if it had not been in the batch.  A gang
+    // whose members carry GPUGangDomain is placed inside the network domain where its members cost least in sum
+    // (kgpu_place_batch_gang_domain has the definition); a member with a gang domain but no gang id, or members of one
+    // gang that disagree, is an error.  `out` is in the caller's order.
     std::string PlaceBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out);
     // Conflict-free PROPOSALS for a whole cycle: like PlaceBatch (each pod sees the GPUs the pods before it would
     // take) but on a scratch copy of the device state -- nothing is taken until TakePodResources commits a pod.
@@ -200,20 +211,20 @@ public:
     // placement and no victims.  (*victims)[p] names the running pods to evict, in name order.  The running pods are the
     // committed placements (PlaceBatch, TakePodResources) until ReturnPodResources; GPUs in use that no committed
     // placement accounts for are never evicted.  Snapshot semantics: nothing is evicted, taken or remembered, two pods
-    // may name the same victims, and gang ids are ignored.
+    // may name the same victims, and gang ids and gang domains are ignored.
     std::string PreemptBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
                              std::vector<std::vector<std::string>> *victims);
     // The conflict-free counterpart of PreemptBatch, as ProposeBatch is of ScoreBatch (kgpu_preempt_plan): pods are
     // taken in the caller's order, each on the state the pods before it leave -- their GPUs taken, their victims' GPUs
     // free, neither evictable again -- so no two pods name the same victim or GPU.  Pass pods in priority order.  Like
-    // PreemptBatch, nothing is evicted, taken or remembered and gang ids are ignored: commit a plan with
+    // PreemptBatch, nothing is evicted, taken or remembered and gang ids and gang domains are ignored: commit a plan with
     // TakePodResources / ReturnPodResources once the victims are gone.
     std::string PlanPreemption(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
                                std::vector<std::vector<std::string>> *victims);
     // PlanPreemption with gangs (GPUGangID, kgpu_preempt_plan_gang): members are moved up to their gang's first member
     // as in PlaceBatch, and a gang evicts and takes all together or not at all.  If one member cannot be placed, the
     // whole gang gets fits = false and no victims, and the pods after it see the victims its other members would have
-    // named as running pods again.  `out` and `victims` are in the caller's order.
+    // named as running pods again.  Gang domains are ignored.  `out` and `victims` are in the caller's order.
     std::string PlanGangPreemption(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
                                    std::vector<std::vector<std::string>> *victims);
     std::string LastError() const { return lastError_; }
@@ -232,6 +243,7 @@ public:
         bool explicitTopo = false;
         bool removed = false;
         std::vector<std::string> owners;      // holder-table owner o -> pod name, as last pushed to the device
+        std::string domain;                   // SetNodeDomain ("" = none)
     };
     const NodeRecord *node(const std::string &nodeName) const;
     static int64_t PodGPUCount(const types::PodInfo &podInfo);     // k of gpu.go:295-303
@@ -246,6 +258,7 @@ private:
     const NodeRecord *recordOf(const types::NodeInfo *nodeInfo) const;
     std::string pushMask(NodeRecord &rec);
     std::string pushHolders();
+    std::string pushDomains();
     TreeCache cache_;
     std::map<std::string, NodeRecord> nodes_;
     std::vector<std::string> indexToName_;
@@ -256,6 +269,7 @@ private:
     std::vector<std::string> changed_;                  // existing nodes whose matrix / presence changed (kgpu_update_node)
     std::set<std::string> holdersChanged_;              // nodes whose running pods changed since the last holder push
     bool holdersReset_ = true;                          // the device table was reset (re-upload): push every row
+    bool domainsDirty_ = false;                         // a node's domain changed, or a re-upload reset the device table
     bool groupSchedulerMode_ = false;
     std::string lastError_;
 };

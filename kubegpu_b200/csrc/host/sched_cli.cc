@@ -10,7 +10,9 @@
 //   addnode NAME KUBEALLOC [key=val ...]        AddNode with Allocatable = {key: val}
 //   rmnode NAME                                 RemoveNode
 //   topo NAME v0 .. v63                         SetNodeTopology (extension)
-//   pod NAME [topogen=V] [minmem=MiB] [gang=ID] [priority=L] {run|init CNAME req=N [kube=N] [dev:key=val ...]}...
+//   domain NODE [NAME]                          SetNodeDomain (extension): the node's network domain, none without NAME
+//   pod NAME [topogen=V] [minmem=MiB] [gang=ID] [gangdomain=required|preferred] [priority=L]
+//       {run|init CNAME req=N [kube=N] [dev:key=val ...]}...
 //   fits NODE POD                               PodFitsDevice  -> fits/score + rewritten requests
 //   allocate NODE POD                           PodAllocate    -> error text + AllocateFrom
 //   take POD | return POD                       TakePodResources / ReturnPodResources
@@ -128,6 +130,11 @@ int main(int argc, char **argv) {
             in >> name;
             for (int i = 0; i < 64; i++) in >> t[i];
             printf("  err=%s\n", sched.SetNodeTopology(name, t).c_str());
+        } else if (cmd == "domain") {
+            std::string name, dom;
+            in >> name;
+            in >> dom;
+            printf("  err=%s\n", sched.SetNodeDomain(name, dom).c_str());
         } else if (cmd == "pod") {
             std::string name, tok, k;
             long long v = 0;
@@ -147,6 +154,11 @@ int main(int argc, char **argv) {
                     pod.Requests[GPUMinMemoryMiB] = atoll(tok.c_str() + 7);
                 } else if (tok.compare(0, 5, "gang=") == 0) {
                     pod.Requests[GPUGangID] = atoll(tok.c_str() + 5);
+                } else if (tok.compare(0, 11, "gangdomain=") == 0) {
+                    const std::string gd = tok.substr(11);
+                    pod.Requests[GPUGangDomain] = gd == "required" ? 1
+                                                  : gd == "preferred" ? 2
+                                                                      : atoll(gd.c_str());
                 } else if (tok.compare(0, 9, "priority=") == 0) {
                     pod.Requests[GPUPriorityLevel] = atoll(tok.c_str() + 9);
                 } else if (cur && tok.compare(0, 4, "req=") == 0) {

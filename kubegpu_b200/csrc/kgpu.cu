@@ -18,6 +18,7 @@
 
 #include "buffer.h"
 #include "multi_device.h"
+#include "gang_domain.cuh"
 #include "place_sequential.cuh"
 #include "preempt.cuh"
 #include "preempt_plan.cuh"
@@ -82,6 +83,12 @@ struct kgpu_shard {
     kgpu::DeviceBuffer<unsigned long long> d_plan_nodekey;   //   per-column node keys [cols][Npad]
     kgpu::DeviceBuffer<unsigned long long> d_plan_tilekey;   //   and their tile minima [cols][T]
     kgpu::DeviceBuffer<int4> d_plan_pre;       // kgpu_preempt_plan_gang: each placed member's pre-image {F, H row} [P]
+    kgpu::DeviceBuffer<int32_t> d_dom_off;     // kgpu_upload_domains: [D + 1] each domain's range of d_dom_nodes,
+    kgpu::DeviceBuffer<int32_t> d_dom_nodes;   //   its nodes in increasing index (nodes of no domain left out)
+    int32_t n_dom = 0;               // D; 0 = every node in no domain (no upload since the last kgpu_upload_nodes)
+    kgpu::DeviceBuffer<int32_t> d_dom_mask;    // domain steps: per-node working mask of the trials [n]
+    kgpu::DeviceBuffer<uint32_t> d_dom_stamp;  //   and the stamp of the trial that wrote it [n]
+    kgpu::DeviceBuffer<unsigned long long> d_dom_best;   //   per step: (C_d << 32 | d) of the best trial
     int64_t class_count[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     int64_t n_slots = 0;
     int64_t n = 0;
@@ -610,6 +617,7 @@ int upload_nodes(kgpu_ctx *h, const int32_t *topo, const int32_t *free_mask, int
         }
         s.n = cnt;
         s.has_hold = false;            // a new node array has no holders
+        s.n_dom = 0;                   // and no domains
         s.node_id_base = node_id_base + off;
         s.order_dirty = true;
         s.compact_dirty = true;
@@ -653,7 +661,7 @@ int kgpu_upload_nodes(kgpu_t *h, const int32_t *topo, const int32_t *free_mask, 
     if (per > 0x7FFFFFFFLL - 4096) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_nodes: more than 2^31 nodes per device");
     const int rc = upload_nodes(h, topo, free_mask, n, node_id_base, per);
     if (rc != KGPU_OK) {               // a failed upload leaves the handle EMPTY (n = 0 everywhere), never half old / half new
-        for (auto &s : h->shards) { s.n = 0; s.n_slots = 0; s.order_dirty = true; s.compact_dirty = true; s.fit_valid = false; s.work_P = -1; }
+        for (auto &s : h->shards) { s.n = 0; s.n_slots = 0; s.n_dom = 0; s.order_dirty = true; s.compact_dirty = true; s.fit_valid = false; s.work_P = -1; }
         h->n_total = 0;
         return rc;
     }
@@ -825,6 +833,55 @@ int kgpu_place_batch_ex(kgpu_t *h, const int32_t *pods, int64_t P, uint64_t *out
 }
 
 int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, int64_t P, uint64_t *out_keys, int flags) {
+    return kgpu_place_batch_gang_domain(h, pods, gang, nullptr, P, out_keys, flags);
+}
+
+namespace {
+// gang_domain: every value 0, REQUIRED or PREFERRED, nonzero only on gang members, the same for all members of a gang,
+// and a constrained gang small enough for the 32-bit cost sum of its trials.
+int check_gang_domain(kgpu_ctx *h, const int32_t *gang, const int32_t *gang_domain, int64_t P) {
+    const char *fn = "kgpu_place_batch_gang_domain";
+    for (int64_t p = 0; p < P; p++) {
+        const int32_t v = gang_domain[p];
+        if (v != 0 && v != KGPU_GANG_DOMAIN_REQUIRED && v != KGPU_GANG_DOMAIN_PREFERRED)
+            return fail(h, KGPU_ERR_INVALID, "%s: gang_domain[%lld] = %d is not 0, REQUIRED (1) or PREFERRED (2)", fn, (long long)p, v);
+        if (v != 0 && (!gang || gang[p] == 0))
+            return fail(h, KGPU_ERR_INVALID, "%s: gang_domain[%lld] = %d on a pod without a gang", fn, (long long)p, v);
+        if (gang && p > 0 && gang[p] != 0 && gang[p] == gang[p - 1] && v != gang_domain[p - 1])
+            return fail(h, KGPU_ERR_INVALID, "%s: the members of gang %d disagree on gang_domain (%d at pod %lld, %d at pod %lld)", fn,
+                        gang[p], gang_domain[p - 1], (long long)(p - 1), v, (long long)p);
+    }
+    for (const kgpu::PlaceSegment &sg : kgpu::place_segments(gang, gang_domain, P))
+        if (sg.mode != 0 && sg.end - sg.begin > kgpu::DOM_MAX_MEMBERS)
+            return fail(h, KGPU_ERR_INVALID, "%s: gang %d has %lld members with a domain constraint, more than %lld", fn, gang[sg.begin],
+                        (long long)(sg.end - sg.begin), (long long)kgpu::DOM_MAX_MEMBERS);
+    return KGPU_OK;
+}
+}  // namespace
+
+int kgpu_upload_domains(kgpu_t *h, const int32_t *domain, int64_t n) {
+    if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_domains: NULL handle");
+    std::lock_guard<std::mutex> g(h->mu);
+    if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_upload_domains: needs a single-device handle");
+    if (n != h->n_total || (n > 0 && !domain)) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_domains: n must equal kgpu_num_nodes");
+    std::vector<int32_t> off, nodes;
+    const int64_t bad = kgpu::domain_lists(domain, n, off, nodes);
+    if (bad >= 0)
+        return fail(h, KGPU_ERR_INVALID, "kgpu_upload_domains: domain[%lld] = %d is neither -1 nor 0..%lld", (long long)bad, domain[bad],
+                    (long long)(n - 1));
+    kgpu_shard &s = h->shards[0];
+    KGPU_CUDA(h, cudaSetDevice(s.dev));
+    KGPU_CUDA(h, s.d_dom_off.reserve((int64_t)off.size()));
+    KGPU_CUDA(h, s.d_dom_nodes.reserve(std::max<int64_t>(1, (int64_t)nodes.size())));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_dom_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice, s.stream));
+    if (!nodes.empty()) KGPU_CUDA(h, cudaMemcpyAsync(s.d_dom_nodes, nodes.data(), nodes.size() * 4, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, cudaStreamSynchronize(s.stream));
+    s.n_dom = (int32_t)(off.size() - 1);
+    return KGPU_OK;
+}
+
+int kgpu_place_batch_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *gang, const int32_t *gang_domain, int64_t P,
+                                 uint64_t *out_keys, int flags) {
     if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_place_batch: NULL handle");
     std::lock_guard<std::mutex> g(h->mu);
     if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_place_batch: needs a single-device handle");
@@ -832,6 +889,10 @@ int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, i
     if (P == 0) return KGPU_OK;
     if (gang) {
         const int rc = check_gang_runs(h, "kgpu_place_batch_gang", gang, P);
+        if (rc != KGPU_OK) return rc;
+    }
+    if (gang_domain) {
+        const int rc = check_gang_domain(h, gang, gang_domain, P);
         if (rc != KGPU_OK) return rc;
     }
     kgpu::PlaceViews views;
@@ -865,22 +926,47 @@ int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, i
             s.d_tilebest, T);
         kgpu::place_half_tables<<<(unsigned)std::min<int64_t>((s.n + 3) / 4, (int64_t)s.sm_count * 16), 128, 0, s.stream>>>(
             s.d_topo, s.n, W, s.d_half);
-        h->launches++;
+        h->launches += 2;
         if (!s.place_attr_done) {          // 72 KB of dynamic shared memory: opt in, once per device
             KGPU_CUDA(h, cudaFuncSetAttribute(kgpu::place_sequential<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kgpu::PLACE_DYN_SMEM));
             KGPU_CUDA(h, cudaFuncSetAttribute(kgpu::place_sequential<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kgpu::PLACE_DYN_SMEM));
             s.place_attr_done = true;
         }
-        if (gang) {
-            kgpu::place_sequential<true><<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(
-                s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base, reinterpret_cast<const int4 *>(s.d_pods.get()), P, W, views,
-                s.d_nodebest, s.d_tilebest, T, s.d_half, s.d_keys, s.d_gang);
-        } else {
-            kgpu::place_sequential<false><<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base,
-                                                                                   reinterpret_cast<const int4 *>(s.d_pods.get()), P, W, views,
-                                                                                   s.d_nodebest, s.d_tilebest, T, s.d_half, s.d_keys);
+        const std::vector<kgpu::PlaceSegment> segs = kgpu::place_segments(gang, gang_domain, P);
+        const int64_t steps = std::count_if(segs.begin(), segs.end(), [](const kgpu::PlaceSegment &sg) { return sg.mode != 0; });
+        kgpu::DomainArgs da = {};
+        if (steps > 0) {               // the trials' scratch: stamps 2 i + 1 (trials of step i) and 2 i + 2 (its commit)
+            KGPU_CUDA(h, s.d_dom_mask.reserve(s.n));
+            KGPU_CUDA(h, s.d_dom_stamp.reserve(s.n));
+            KGPU_CUDA(h, s.d_dom_best.reserve(steps, pod_headroom(steps)));
+            if (s.n_dom == 0) KGPU_CUDA(h, s.d_dom_off.reserve(1));
+            KGPU_CUDA(h, cudaMemsetAsync(s.d_dom_stamp, 0, (size_t)s.n * 4, s.stream));
+            KGPU_CUDA(h, cudaMemsetAsync(s.d_dom_best, 0xFF, (size_t)steps * 8, s.stream));
+            da = kgpu::DomainArgs{d_free, s.d_mem, Npad, T, s.node_id_base, views, s.d_nodebest, s.d_tilebest, s.d_half,
+                                  s.d_dom_off, s.d_dom_nodes, s.d_dom_mask, s.d_dom_stamp};
         }
-        h->launches += 2;
+        const int4 *pods4 = reinterpret_cast<const int4 *>(s.d_pods.get());
+        int64_t step = 0;
+        for (const kgpu::PlaceSegment &sg : segs) {
+            const int64_t p0 = sg.begin, np = sg.end - sg.begin;
+            if (sg.mode != 0) {
+                const uint32_t stamp = (uint32_t)(2 * step + 1);
+                kgpu::domain_trial<<<kgpu::domain_trial_blocks(s.n_dom, (int64_t)s.sm_count * 8), kgpu::DOM_THREADS, 0, s.stream>>>(
+                    da, pods4 + p0, np, s.n_dom, stamp, s.d_dom_best + step);
+                kgpu::domain_commit<<<1, kgpu::DOM_COMMIT_THREADS, 0, s.stream>>>(da, pods4 + p0, np, sg.mode, stamp + 1,
+                                                                                 s.d_dom_best + step, s.d_keys + p0);
+                step++;
+            } else if (gang) {
+                kgpu::place_sequential<true><<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(
+                    s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base, pods4 + p0, np, W, views, s.d_nodebest, s.d_tilebest, T,
+                    s.d_half, s.d_keys + p0, s.d_gang + p0);
+            } else {
+                kgpu::place_sequential<false><<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(
+                    s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base, pods4 + p0, np, W, views, s.d_nodebest, s.d_tilebest, T,
+                    s.d_half, s.d_keys + p0);
+            }
+            h->launches += sg.mode != 0 ? 2 : 1;
+        }
         if (!dry) {
             s.order_dirty = true;        // the free masks have changed on the device: re-sort + recompact lazily
             s.fit_valid = false;

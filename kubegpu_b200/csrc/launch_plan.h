@@ -9,6 +9,7 @@
 #include <utility>
 #include <vector>
 
+#include "gang_domain.cuh"
 #include "place_sequential.cuh"
 #include "score_pairs_sparse.cuh"
 #include "sparse_work.h"
@@ -41,6 +42,57 @@ inline bool place_views(const int32_t *pods, int64_t P, PlaceViews &views) {
         views.min_mem[views.n++] = need;
     }
     return true;
+}
+
+// kgpu_place_batch_gang_domain: the batch cut into segments, in order.  A constrained gang (a run of consecutive pods with
+// the same nonzero gang id and a nonzero gang_domain, which the host has checked its members agree on) is one domain
+// step, mode = its gang_domain: domain_trial + domain_commit.  Every maximal pod range without one is one place_sequential
+// launch on pods + begin, mode = 0.  gang_domain == nullptr (or all 0): one segment, the whole batch.
+struct PlaceSegment {
+    int64_t begin, end;
+    int32_t mode;
+};
+inline std::vector<PlaceSegment> place_segments(const int32_t *gang, const int32_t *gang_domain, int64_t P) {
+    std::vector<PlaceSegment> seg;
+    int64_t p = 0, plain = 0;
+    while (p < P) {
+        if (gang_domain == nullptr || gang_domain[p] == 0) {
+            p++;
+            continue;
+        }
+        int64_t e = p + 1;
+        while (e < P && gang[e] == gang[p]) e++;
+        if (plain < p) seg.push_back({plain, p, 0});
+        seg.push_back({p, e, gang_domain[p]});
+        p = plain = e;
+    }
+    if (plain < P) seg.push_back({plain, P, 0});
+    return seg;
+}
+
+// kgpu_upload_domains: the node lists of the domains in one counting pass.  domain[n] is -1 (no domain) or 0..n-1;
+// D = 1 + the largest id.  off[D + 1]; nodes[] holds each domain's nodes in increasing index, -1 nodes left out.
+// Returns the index of the first value outside -1..n-1 (nothing built), or -1.
+inline int64_t domain_lists(const int32_t *domain, int64_t n, std::vector<int32_t> &off, std::vector<int32_t> &nodes) {
+    int32_t D = 0;
+    for (int64_t i = 0; i < n; i++) {
+        if (domain[i] < -1 || domain[i] >= n) return i;
+        D = std::max(D, domain[i] + 1);
+    }
+    off.assign((size_t)D + 1, 0);
+    for (int64_t i = 0; i < n; i++)
+        if (domain[i] >= 0) off[(size_t)domain[i] + 1]++;
+    for (int32_t d = 0; d < D; d++) off[(size_t)d + 1] += off[(size_t)d];
+    nodes.assign((size_t)off[(size_t)D], 0);
+    std::vector<int32_t> at(off.begin(), off.end() - 1);
+    for (int64_t i = 0; i < n; i++)
+        if (domain[i] >= 0) nodes[(size_t)at[(size_t)domain[i]]++] = (int32_t)i;
+    return -1;
+}
+
+// domain_trial's grid: warp per domain, at most max_blocks blocks (grid-strided beyond), at least one
+inline unsigned domain_trial_blocks(int64_t D, int64_t max_blocks) {
+    return (unsigned)std::max<int64_t>(1, std::min<int64_t>((D + DOM_WARPS - 1) / DOM_WARPS, max_blocks));
 }
 
 // Preemption plans: the batch's columns, the distinct (k, level, min_mem) with k in 1..8, sorted (k first, so warps stay

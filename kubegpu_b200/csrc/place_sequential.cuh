@@ -197,6 +197,20 @@ __device__ __forceinline__ unsigned long long warp_min_u64_redux(unsigned long l
     return ((unsigned long long)mhi << 32) | mlo;
 }
 
+// Tile minimum of one (view, k) row, as the refresh computes it: every lane folds the node keys of its nodes of the tile
+// (offset `off` in the tile) into a 32-bit composite cost << 15 | node offset << 8 | S (cost <= 28 * 4095 < 2^17), and
+// tile_min_key takes the warp's minimum with one REDUX and widens it to the 64-bit key.
+__device__ __forceinline__ uint32_t tile_fold(uint32_t m, uint32_t key, int off) {
+    if (key != INF32) m = min(m, ((key >> 8) << 15) | ((uint32_t)off << 8) | (key & 0xFFu));
+    return m;
+}
+__device__ __forceinline__ unsigned long long tile_min_key(uint32_t m, int64_t node_id_base, int tile) {
+    m = __reduce_min_sync(0xFFFFFFFFu, m);
+    return m == INF32 ? ~0ull
+                      : (((unsigned long long)(m >> 15) << 40) |
+                         ((unsigned long long)(node_id_base + (int64_t)tile * PLACE_TILE + ((m >> 8) & 127u)) << 8) | (m & 0xFFu));
+}
+
 constexpr int PLACE_POD_CHUNK = 1024;       // pod requests staged in shared memory (16 KB)
 constexpr size_t PLACE_DYN_SMEM = 2 * (size_t)PLACE_SUPER_CAP * sizeof(unsigned long long);
 
@@ -405,7 +419,6 @@ place_sequential(const int32_t *__restrict__ topo, int32_t *__restrict__ free_ma
                         }
                         const uint32_t ok = tv == 0 ? 0xFFu : (__ballot_sync(0xFFFFFFFFu, c_mem >= sViewMin[tv]) & 0xFFu);
                         const uint32_t nk = node_key_warp(tk, half, fm & ok, lane, sSub[tk], sNsub[tk]);
-                        // tile minimum: 32-bit composite cost << 15 | node offset << 8 | S (cost <= 28 * 4095 < 2^17)
                         uint32_t m = INF32;
 #pragma unroll
                         for (int j = 0; j < PLACE_TILE / 32; j++) {
@@ -415,13 +428,9 @@ place_sequential(const int32_t *__restrict__ topo, int32_t *__restrict__ free_ma
                                 key = nk;
                                 if (cached) nbr[j] = nk;
                             }
-                            if (key != INF32) m = min(m, ((key >> 8) << 15) | ((uint32_t)off << 8) | (key & 0xFFu));
+                            m = tile_fold(m, key, off);
                         }
-                        m = __reduce_min_sync(0xFFFFFFFFu, m);
-                        const unsigned long long tb =
-                            m == INF32 ? ~0ull
-                                       : (((unsigned long long)(m >> 15) << 40) |
-                                          ((unsigned long long)(node_id_base + (int64_t)tile * PLACE_TILE + ((m >> 8) & 127u)) << 8) | (m & 0xFFu));
+                        const unsigned long long tb = tile_min_key(m, node_id_base, tile);
                         if (cached && cache_super) {
                             if (lane == (tile & 31)) tsr = tb;
                             sb = warp_min_u64_redux(tsr);

@@ -146,25 +146,45 @@ class Scorer:
         self._check(self._L.kgpu_score_batch(self._h, pods.ctypes.data, P, out.ctypes.data))
         return out
 
-    def place_batch(self, pods, out: Optional[np.ndarray] = None, dry_run: bool = False, gang=None) -> np.ndarray:
+    def place_batch(self, pods, out: Optional[np.ndarray] = None, dry_run: bool = False, gang=None,
+                    gang_domain=None) -> np.ndarray:
         """Stateful sequential placement: pods in order, each takes its GPUs (device free masks change).
         dry_run: conflict-free proposals on a scratch copy of the masks, the handle's state is untouched.
         gang: int32[P] gang ids, 0 = the pod is on its own.  A run of consecutive pods with the same nonzero id
         is placed all or nothing: if a member does not fit, the members before it give their GPUs back and the
-        whole gang gets NO_FIT.  An id in two separate runs raises KgpuError (ERR_INVALID)."""
+        whole gang gets NO_FIT.  An id in two separate runs raises KgpuError (ERR_INVALID).
+        gang_domain: int32[P], 0 = no constraint, 1 (GANG_DOMAIN_REQUIRED) = the gang is placed inside one domain of
+        upload_domains or not at all, 2 (GANG_DOMAIN_PREFERRED) = inside one domain if one fits, else as a plain gang.
+        Nonzero only on gang members, the same for every member of a gang (include/kgpu.h has the definition)."""
         pods = _i32(pods)
         P = pods.size // 4
         if out is None:
             out = np.empty(P, dtype=np.uint64)
         flags = _lib.PLACE_DRY_RUN if dry_run else 0
-        if gang is None:
+        if gang is None and gang_domain is None:
             self._check(self._L.kgpu_place_batch_ex(self._h, pods.ctypes.data, P, out.ctypes.data, flags))
             return out
-        gang = _i32(gang)
-        if gang.size != P:
-            raise ValueError("gang must hold one id per pod")
-        self._check(self._L.kgpu_place_batch_gang(self._h, pods.ctypes.data, gang.ctypes.data, P, out.ctypes.data, flags))
+        if gang is not None:
+            gang = _i32(gang)
+            if gang.size != P:
+                raise ValueError("gang must hold one id per pod")
+        if gang_domain is None:
+            self._check(self._L.kgpu_place_batch_gang(self._h, pods.ctypes.data, gang.ctypes.data, P, out.ctypes.data, flags))
+            return out
+        gang_domain = _i32(gang_domain)
+        if gang_domain.size != P:
+            raise ValueError("gang_domain must hold one value per pod")
+        self._check(self._L.kgpu_place_batch_gang_domain(self._h, pods.ctypes.data, None if gang is None else gang.ctypes.data,
+                                                         gang_domain.ctypes.data, P, out.ctypes.data, flags))
         return out
+
+    def upload_domains(self, domain) -> None:
+        """domain[N]: each node's network domain, -1 (none) or 0..N-1 (the nodes under one leaf switch, one scalable
+        unit or one NVLink Switch domain).  Until the first upload, and after upload_nodes, every node is in none."""
+        dom = _i32(domain)
+        if dom.size != self.num_nodes:
+            raise ValueError("domain must hold one value per node")
+        self._check(self._L.kgpu_upload_domains(self._h, dom.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), dom.size))
 
     # -- preemption (PostFilter) -----------------------------------------------------
     def upload_holders(self, holders) -> None:

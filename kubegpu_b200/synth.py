@@ -240,3 +240,15 @@ def gen_gangs(N: int = 100_000, P: int = 10_000, seed: int = SEED_GANGS, gang_st
         else:
             p += 1
     return topo, free, pods, gang
+
+
+SEED_DOMAINS = 0xB200000A
+
+
+def gen_domains(N: int, size: int, seed: int = SEED_DOMAINS) -> np.ndarray:
+    """Network domains for N nodes: the nodes dealt into domains of ``size`` (the last one may be smaller) by a seeded
+    permutation, so a domain is not a contiguous index range.  Returns int32[N], ids 0 .. ceil(N / size) - 1."""
+    order = np.argsort(rand_u64(seed, 31, N), kind="stable")
+    dom = np.empty(N, dtype=np.int32)
+    dom[order] = (np.arange(N) // size).astype(np.int32)
+    return dom
