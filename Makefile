@@ -22,7 +22,7 @@ $(HOSTLIB): $(CSRC)/host/device_scheduler.cc $(CSRC)/host/gpus_info.cc $(CSRC)/h
 $(CLI): $(CSRC)/host/sched_cli.cc $(HOSTLIB)
 	$(CXX) $(CXXFLAGS) -o $@ $(CSRC)/host/sched_cli.cc -Lkubegpu_b200/lib -lkgpu_host -lkgpu -Wl,-rpath,'$$ORIGIN'
 
-$(LIB): $(CSRC)/kgpu.cu $(CSRC)/buffer.h $(CSRC)/score_pairs.cuh $(CSRC)/place_sequential.cuh $(CSRC)/gang_domain.cuh $(CSRC)/preempt.cuh $(CSRC)/preempt_plan.cuh $(CSRC)/score_pairs_sparse.cuh $(CSRC)/sparse_work.h $(CSRC)/launch_plan.h $(CSRC)/peer_exchange.cuh $(CSRC)/node_state.cuh $(CSRC)/subset_dp_sparse_gen.cuh $(CSRC)/subset_dp_gen.cuh $(CSRC)/multi_device.cc $(CSRC)/multi_device.h include/kgpu.h
+$(LIB): $(CSRC)/kgpu.cu $(CSRC)/buffer.h $(CSRC)/score_pairs.cuh $(CSRC)/place_sequential.cuh $(CSRC)/gang_domain.cuh $(CSRC)/preempt.cuh $(CSRC)/preempt_plan.cuh $(CSRC)/preempt_plan_domain.cuh $(CSRC)/score_pairs_sparse.cuh $(CSRC)/sparse_work.h $(CSRC)/launch_plan.h $(CSRC)/peer_exchange.cuh $(CSRC)/node_state.cuh $(CSRC)/subset_dp_sparse_gen.cuh $(CSRC)/subset_dp_gen.cuh $(CSRC)/multi_device.cc $(CSRC)/multi_device.h include/kgpu.h
 	@mkdir -p kubegpu_b200/lib
 	$(NVCC) $(NVCCFLAGS) -shared -o $@ $(CSRC)/kgpu.cu $(CSRC)/multi_device.cc -ldl
 

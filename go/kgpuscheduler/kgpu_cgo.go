@@ -253,3 +253,26 @@ func (k *handle) preemptPlanGang(pods []int32, lvl []int32, gang []int32) ([]uin
 	}
 	return keys, victims, nil
 }
+
+// preemptPlanDomain: preemptPlanGang with gang domains (kgpu_preempt_plan_gang_domain, gangDomain as for
+// placeBatchDomain): a REQUIRED gang evicts and takes its GPUs inside one domain of uploadDomains or gets NO_FIT; a
+// PREFERRED gang falls back to the plain gang plan.  gang may be nil when every gangDomain value is 0.
+func (k *handle) preemptPlanDomain(pods []int32, lvl []int32, gang []int32, gangDomain []int32) ([]uint64, []uint32, error) {
+	keys := make([]uint64, len(pods)/4)
+	victims := make([]uint32, len(keys))
+	if len(keys) == 0 {
+		return keys, victims, nil
+	}
+	var g, gd *C.int32_t
+	if gang != nil {
+		g = (*C.int32_t)(unsafe.Pointer(&gang[0]))
+	}
+	if gangDomain != nil {
+		gd = (*C.int32_t)(unsafe.Pointer(&gangDomain[0]))
+	}
+	if rc := C.kgpu_preempt_plan_gang_domain(k.h, (*C.int32_t)(unsafe.Pointer(&pods[0])), (*C.int32_t)(unsafe.Pointer(&lvl[0])), g, gd,
+		C.int64_t(len(keys)), (*C.uint64_t)(unsafe.Pointer(&keys[0])), (*C.uint32_t)(unsafe.Pointer(&victims[0]))); rc != C.KGPU_OK {
+		return nil, nil, k.err("kgpu_preempt_plan_gang_domain")
+	}
+	return keys, victims, nil
+}

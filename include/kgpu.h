@@ -295,6 +295,38 @@ int kgpu_preempt_plan(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_
  * single-device handles, host buffers and synchronous, as for kgpu_preempt_plan. */
 int kgpu_preempt_plan_gang(kgpu_t *h, const int32_t *pods, const int32_t *lvl, const int32_t *gang, int64_t P,
                            uint64_t *out_keys, uint32_t *out_victims);
+/* kgpu_preempt_plan_gang inside one network domain: a constrained gang evicts and takes its GPUs within one domain of
+ * kgpu_upload_domains, so a plan never kills running pods for a gang that placement would then refuse.  Arguments,
+ * output format, limits and dry-run semantics as for kgpu_preempt_plan_gang; gang_domain[P] as for
+ * kgpu_place_batch_gang_domain (0, KGPU_GANG_DOMAIN_REQUIRED or KGPU_GANG_DOMAIN_PREFERRED); the domain table and its
+ * lifetime as there.  (F, H) starts as the handle's free masks and holder table, and the pods are taken in order.  Pods
+ * and gangs with gang_domain 0 are taken exactly as by kgpu_preempt_plan_gang.  A CONSTRAINED gang m1..mj:
+ *   1. Trial per domain.  Every domain d with at least one node gets a trial on a copy (F_d, H_d): for i = 1..j, if
+ *      k(m_i) is outside 0..8 the trial fails; a k = 0 member costs 0, evicts nothing, takes nothing and gets the
+ *      domain's lowest node; otherwise m_i gets what kgpu_preempt_batch would give it alone on (F_d, H_d) restricted to
+ *      the nodes with domain[n] = d (the minimum candidate in the order (max victim level, |V|, cost, node id, S), with
+ *      min_mem_mib applied as in scoring); with no candidate the trial fails, otherwise the update rule of
+ *      kgpu_preempt_plan is applied to (F_d, H_d).  A trial that places every member has the score (L_d, V_d, C_d):
+ *      L_d the largest victim level over the members that evict (0 if none does), V_d the total victim count (victim
+ *      sets are disjoint), C_d the sum of the members' costs.  So a trial that evicts nothing ranks before one that
+ *      evicts level-0 pods.
+ *   2. Choice.  If some trial succeeded, the gang takes the domain with the smallest (L_d, V_d, C_d, d): (F, H) becomes
+ *      that trial's (F_d, H_d), and the members get its keys and victims.
+ *   3. No domain fits, REQUIRED: every member gets KGPU_NO_FIT and victims 0; (F, H) is unchanged.
+ *   4. No domain fits, PREFERRED: the gang is taken exactly as kgpu_preempt_plan_gang would take it on (F, H): over all
+ *      nodes, all or nothing.
+ * Consequences: P1 gang_domain == NULL (or all 0) is kgpu_preempt_plan_gang, with the same kernel launches; P2 with
+ * every node in domain 0, REQUIRED and PREFERRED both are kgpu_preempt_plan_gang; P3 without a holder table, or with
+ * every lvl 0, the keys equal kgpu_place_batch_gang_domain(KGPU_PLACE_DRY_RUN) on the same domain table and every
+ * victim mask is 0; P4 the members of a placed REQUIRED gang and all their victims sit on the nodes of one domain,
+ * never on a node of domain -1; P5 PREFERRED gives the REQUIRED result when some domain fits, the plain gang result
+ * otherwise; P6 a failed REQUIRED gang leaves (F, H) as it was, so the result equals the call on the batch with that
+ * gang deleted.
+ * KGPU_ERR_INVALID, checked before anything runs: the checks of kgpu_preempt_plan_gang and the gang_domain checks of
+ * kgpu_place_batch_gang_domain (values, members that agree, at most 37 000 members per constrained gang).  Dry run
+ * only; single-device handles (KGPU_ERR_STATE otherwise).  Host buffers, synchronous. */
+int kgpu_preempt_plan_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *lvl, const int32_t *gang,
+                                  const int32_t *gang_domain, int64_t P, uint64_t *out_keys, uint32_t *out_victims);
 /* Copy the current free masks (n = kgpu_num_nodes entries) back to the host. */
 int kgpu_get_free_masks(kgpu_t *h, int32_t *out_free_mask, int64_t n);
 

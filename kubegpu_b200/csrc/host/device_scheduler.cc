@@ -615,6 +615,11 @@ std::string NvidiaGPUScheduler::PlanGangPreemption(const std::vector<const types
     return runBatch(pods, out, BatchMode::PreemptGangPlan, victims);
 }
 
+std::string NvidiaGPUScheduler::PlanGangDomainPreemption(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
+                                                         std::vector<std::vector<std::string>> *victims) {
+    return runBatch(pods, out, BatchMode::PreemptGangDomainPlan, victims);
+}
+
 // Holder rows from the committed placements: on each node the pods holding GPUs, in name order, are owners 0, 1, ...;
 // a GPU gets level << 3 | owner of the pod that holds it, -1 if no committed placement accounts for it.  Pushed for the
 // nodes changed since the last push (kgpu_set_holders), or all of them after a re-upload reset the table.
@@ -669,7 +674,7 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     std::vector<int32_t> gang, gangDomain;          // gangDomain: in device order, empty when no pod asks for a domain
     for (size_t p = 0; p < P; p++) order[p] = p;
     const bool placing = mode == BatchMode::Sequential || mode == BatchMode::DryRun;
-    if (placing) {
+    if (placing || mode == BatchMode::PreemptGangDomainPlan) {
         std::map<int64_t, int64_t> domainOfGang;
         for (size_t p = 0; p < P; p++) {
             const int64_t gd = getOr0(pods[p]->Requests, GPUGangDomain), id = getOr0(pods[p]->Requests, GPUGangID);
@@ -683,7 +688,7 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
         err = pushDomains();
         if (!err.empty()) return err;
     }
-    if (placing || mode == BatchMode::PreemptGangPlan) {
+    if (placing || mode == BatchMode::PreemptGangPlan || mode == BatchMode::PreemptGangDomainPlan) {
         std::map<int64_t, int32_t> dense;
         std::vector<std::vector<size_t>> members;
         std::vector<int32_t> gangOf(P, 0);
@@ -729,7 +734,8 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     std::vector<uint64_t> dev(P, KGPU_NO_FIT);
     std::vector<uint32_t> owners(P, 0);
     std::vector<int32_t> lvl(P, 0);
-    const bool preempt = mode == BatchMode::Preempt || mode == BatchMode::PreemptPlan || mode == BatchMode::PreemptGangPlan;
+    const bool preempt = mode == BatchMode::Preempt || mode == BatchMode::PreemptPlan || mode == BatchMode::PreemptGangPlan ||
+                         mode == BatchMode::PreemptGangDomainPlan;
     if (preempt) {
         for (size_t i = 0; i < P; i++) lvl[i] = levelOf(*pods[order[i]]);
         err = pushHolders();
@@ -740,6 +746,10 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
                    : mode == BatchMode::PreemptGangPlan
                        ? kgpu_preempt_plan_gang(handle_, req.data(), lvl.data(), gang.empty() ? nullptr : gang.data(), (int64_t)P,
                                                 dev.data(), owners.data())
+                   : mode == BatchMode::PreemptGangDomainPlan
+                       ? kgpu_preempt_plan_gang_domain(handle_, req.data(), lvl.data(), gang.empty() ? nullptr : gang.data(),
+                                                       gangDomain.empty() ? nullptr : gangDomain.data(), (int64_t)P, dev.data(),
+                                                       owners.data())
                    : mode == BatchMode::Snapshot ? kgpu_score_batch(handle_, req.data(), (int64_t)P, dev.data())
                                                : kgpu_place_batch_gang_domain(handle_, req.data(), gang.empty() ? nullptr : gang.data(),
                                                                               gangDomain.empty() ? nullptr : gangDomain.data(), (int64_t)P,

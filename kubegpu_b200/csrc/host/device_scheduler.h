@@ -227,6 +227,13 @@ public:
     // named as running pods again.  Gang domains are ignored.  `out` and `victims` are in the caller's order.
     std::string PlanGangPreemption(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
                                    std::vector<std::vector<std::string>> *victims);
+    // PlanGangPreemption inside one network domain (kgpu_preempt_plan_gang_domain): a gang whose members carry
+    // GPUGangDomain evicts and takes its GPUs inside the domain (SetNodeDomain) whose plan is best in (highest victim
+    // level, victim count, summed cost, domain id); with none, a required gang gets fits = false and no victims, a
+    // preferred one is planned as by PlanGangPreemption.  The domain table is pushed as for PlaceBatch, members move
+    // up to their gang's first member, and bad gang domains are errors as there.  Nothing is taken or remembered.
+    std::string PlanGangDomainPreemption(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out,
+                                         std::vector<std::vector<std::string>> *victims);
     std::string LastError() const { return lastError_; }
     const TreeCache &cache() const { return cache_; }
     bool hasDevice() const { return handle_ != nullptr; }
@@ -252,7 +259,7 @@ private:
     std::string syncNode(const NodeRecord &rec);
     std::string flushNodes();
     std::string scoreOne(const NodeRecord &rec, int k, int32_t minMemMiB, uint32_t *nodeKey);
-    enum class BatchMode { Snapshot, Sequential, DryRun, Preempt, PreemptPlan, PreemptGangPlan };
+    enum class BatchMode { Snapshot, Sequential, DryRun, Preempt, PreemptPlan, PreemptGangPlan, PreemptGangDomainPlan };
     std::string runBatch(const std::vector<const types::PodInfo *> &pods, std::vector<Placement> *out, BatchMode mode,
                          std::vector<std::vector<std::string>> *victims = nullptr);
     const NodeRecord *recordOf(const types::NodeInfo *nodeInfo) const;

@@ -22,6 +22,7 @@
 //   preemptbatch POD...                         PreemptBatch (GPU): placements when lower-priority pods may be evicted
 //   preemptplan POD...                          PlanPreemption (GPU): the same in order, no victim or GPU named twice
 //   preemptgangplan POD...                      PlanGangPreemption (GPU): preemptplan with gangs, all members or none
+//   preemptdomainplan POD...                    PlanGangDomainPreemption (GPU): preemptgangplan with gang domains
 //   addjson NAME FILE [nvml]                    AddNodeFromGpusInfo (node agent JSON), dumps names + matrix
 //   visible POD                                 NVIDIA_VISIBLE_DEVICES per container (node agent Allocate)
 //   cache                                       dump the tree cache
@@ -205,7 +206,8 @@ int main(int argc, char **argv) {
             for (size_t i = 0; i < out.size(); i++)
                 printf("  %s fits=%d cost=%u node=%s mask=0x%02x\n", pods[i]->Name.c_str(), out[i].fits ? 1 : 0, out[i].cost,
                        out[i].nodeName.c_str(), out[i].gpuMask);
-        } else if (cmd == "preemptbatch" || cmd == "preemptplan" || cmd == "preemptgangplan") {
+        } else if (cmd == "preemptbatch" || cmd == "preemptplan" || cmd == "preemptgangplan" ||
+                   cmd == "preemptdomainplan") {
             std::vector<const types::PodInfo *> pods;
             std::string podName;
             while (in >> podName)
@@ -214,6 +216,7 @@ int main(int argc, char **argv) {
             std::vector<std::vector<std::string>> victims;
             const std::string err = cmd == "preemptplan"       ? sched.PlanPreemption(pods, &out, &victims)
                                     : cmd == "preemptgangplan" ? sched.PlanGangPreemption(pods, &out, &victims)
+                                    : cmd == "preemptdomainplan" ? sched.PlanGangDomainPreemption(pods, &out, &victims)
                                                                : sched.PreemptBatch(pods, &out, &victims);
             printf("  err=%s\n", err.c_str());
             for (size_t i = 0; i < out.size(); i++) {

@@ -22,6 +22,7 @@
 #include "place_sequential.cuh"
 #include "preempt.cuh"
 #include "preempt_plan.cuh"
+#include "preempt_plan_domain.cuh"
 #include "sparse_work.h"
 #include "peer_exchange.cuh"
 #include "score_pairs.cuh"
@@ -89,6 +90,8 @@ struct kgpu_shard {
     kgpu::DeviceBuffer<int32_t> d_dom_mask;    // domain steps: per-node working mask of the trials [n]
     kgpu::DeviceBuffer<uint32_t> d_dom_stamp;  //   and the stamp of the trial that wrote it [n]
     kgpu::DeviceBuffer<unsigned long long> d_dom_best;   //   per step: (C_d << 32 | d) of the best trial
+    kgpu::DeviceBuffer<uint2> d_dom_hold;      // plan domain steps: per-node working holder row of the trials [n]
+    kgpu::DeviceBuffer<unsigned long long> d_dom_score;  //   and each domain's trial score [D]
     int64_t class_count[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     int64_t n_slots = 0;
     int64_t n = 0;
@@ -838,9 +841,8 @@ int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, i
 
 namespace {
 // gang_domain: every value 0, REQUIRED or PREFERRED, nonzero only on gang members, the same for all members of a gang,
-// and a constrained gang small enough for the 32-bit cost sum of its trials.
-int check_gang_domain(kgpu_ctx *h, const int32_t *gang, const int32_t *gang_domain, int64_t P) {
-    const char *fn = "kgpu_place_batch_gang_domain";
+// and a constrained gang small enough for the 32-bit cost sum of its trials.  fn names the entry point in the messages.
+int check_gang_domain(kgpu_ctx *h, const char *fn, const int32_t *gang, const int32_t *gang_domain, int64_t P) {
     for (int64_t p = 0; p < P; p++) {
         const int32_t v = gang_domain[p];
         if (v != 0 && v != KGPU_GANG_DOMAIN_REQUIRED && v != KGPU_GANG_DOMAIN_PREFERRED)
@@ -892,7 +894,7 @@ int kgpu_place_batch_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *
         if (rc != KGPU_OK) return rc;
     }
     if (gang_domain) {
-        const int rc = check_gang_domain(h, gang, gang_domain, P);
+        const int rc = check_gang_domain(h, "kgpu_place_batch_gang_domain", gang, gang_domain, P);
         if (rc != KGPU_OK) return rc;
     }
     kgpu::PlaceViews views;
@@ -1150,9 +1152,12 @@ int plan_columns(kgpu_ctx *h, const char *fn, const int32_t *pods, const int32_t
 }
 
 // The plan's kernels on the working state (F, H), once the batch is on the device (d_pods, d_plan_pcol and, with gangs,
-// d_gang), then the results back to the host.  The handle's masks and holder table are never written.
-int plan_launch(kgpu_ctx *h, kgpu_shard &s, int64_t P, const std::vector<int4> &cols, bool gang, uint64_t *out_keys,
-                uint32_t *out_victims) {
+// d_gang and d_plan_pre), then the results back to the host.  segs (launch_plan.h: place_segments) cut the batch: each
+// range without a constrained gang is one plan_sequential (gang_plan_sequential with gangs) launch on its pods, each
+// constrained gang one domain step, domain_plan_trial + domain_plan_commit.  The handle's masks and holder table are
+// never written.
+int plan_launch(kgpu_ctx *h, kgpu_shard &s, int64_t P, const std::vector<int4> &cols, bool gang,
+                const std::vector<kgpu::PlaceSegment> &segs, uint64_t *out_keys, uint32_t *out_victims) {
     const int ncol = (int)cols.size();
     KGPU_CUDA(h, cudaEventRecord(s.ev0, s.stream));
     if (s.n == 0) {
@@ -1179,17 +1184,45 @@ int plan_launch(kgpu_ctx *h, kgpu_shard &s, int64_t P, const std::vector<int4> &
                 s.d_plan_tilekey);
             h->launches++;
         }
-        if (gang)
-            kgpu::gang_plan_sequential<<<1, kgpu::PLAN_THREADS, 0, s.stream>>>(
-                reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_plan_free, reinterpret_cast<const int4 *>(s.d_mem.get()),
-                s.d_plan_hold, s.n, Npad, T, s.node_id_base, reinterpret_cast<const int4 *>(s.d_pods.get()), s.d_plan_pcol, P,
-                s.d_plan_cols, ncol, W, PC, s.d_plan_nodekey, s.d_plan_tilekey, s.d_keys, s.d_victims, s.d_gang, s.d_plan_pre);
-        else
-            kgpu::plan_sequential<<<1, kgpu::PLAN_THREADS, 0, s.stream>>>(
-                reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_plan_free, reinterpret_cast<const int4 *>(s.d_mem.get()),
-                s.d_plan_hold, s.n, Npad, T, s.node_id_base, reinterpret_cast<const int4 *>(s.d_pods.get()), s.d_plan_pcol, P,
-                s.d_plan_cols, ncol, W, PC, s.d_plan_nodekey, s.d_plan_tilekey, s.d_keys, s.d_victims);
-        h->launches++;
+        const int64_t steps = std::count_if(segs.begin(), segs.end(), [](const kgpu::PlaceSegment &sg) { return sg.mode != 0; });
+        kgpu::PlanDomainArgs da = {};
+        if (steps > 0) {               // the trials' scratch: stamps 2 i + 1 (trials of step i) and 2 i + 2 (its commit)
+            KGPU_CUDA(h, s.d_dom_mask.reserve(s.n));
+            KGPU_CUDA(h, s.d_dom_hold.reserve(s.n));
+            KGPU_CUDA(h, s.d_dom_stamp.reserve(s.n));
+            KGPU_CUDA(h, s.d_dom_score.reserve(std::max<int64_t>(1, s.n_dom)));
+            if (s.n_dom == 0) KGPU_CUDA(h, s.d_dom_off.reserve(1));
+            KGPU_CUDA(h, cudaMemsetAsync(s.d_dom_stamp, 0, (size_t)s.n * 4, s.stream));
+            da = kgpu::PlanDomainArgs{reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_plan_free,
+                                      reinterpret_cast<const int4 *>(s.d_mem.get()), s.d_plan_hold, s.n, Npad, T, s.node_id_base,
+                                      s.d_plan_cols, ncol, s.d_plan_nodekey, s.d_plan_tilekey, s.d_dom_off, s.d_dom_nodes,
+                                      s.d_dom_mask, s.d_dom_hold, s.d_dom_stamp};
+        }
+        const int4 *pods4 = reinterpret_cast<const int4 *>(s.d_pods.get());
+        int64_t step = 0;
+        for (const kgpu::PlaceSegment &sg : segs) {
+            const int64_t p0 = sg.begin, np = sg.end - sg.begin;
+            if (sg.mode != 0) {
+                const uint32_t stamp = (uint32_t)(2 * step + 1);
+                kgpu::domain_plan_trial<<<kgpu::domain_trial_blocks(s.n_dom, (int64_t)s.sm_count * 8), kgpu::DOM_THREADS, 0, s.stream>>>(
+                    da, W, PC, pods4 + p0, s.d_plan_pcol + p0, np, s.n_dom, stamp, s.d_dom_score);
+                kgpu::domain_plan_commit<<<1, kgpu::PLAN_THREADS, 0, s.stream>>>(
+                    da, W, PC, pods4 + p0, s.d_plan_pcol + p0, s.d_gang + p0, np, sg.mode, s.n_dom, stamp + 1, s.d_dom_score,
+                    s.d_keys + p0, s.d_victims + p0, s.d_plan_pre + p0);
+                step++;
+            } else if (gang) {
+                kgpu::gang_plan_sequential<<<1, kgpu::PLAN_THREADS, 0, s.stream>>>(
+                    reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_plan_free, reinterpret_cast<const int4 *>(s.d_mem.get()),
+                    s.d_plan_hold, s.n, Npad, T, s.node_id_base, pods4 + p0, s.d_plan_pcol + p0, np, s.d_plan_cols, ncol, W, PC,
+                    s.d_plan_nodekey, s.d_plan_tilekey, s.d_keys + p0, s.d_victims + p0, s.d_gang + p0, s.d_plan_pre + p0);
+            } else {
+                kgpu::plan_sequential<<<1, kgpu::PLAN_THREADS, 0, s.stream>>>(
+                    reinterpret_cast<const int4 *>(s.d_topo.get()), s.d_plan_free, reinterpret_cast<const int4 *>(s.d_mem.get()),
+                    s.d_plan_hold, s.n, Npad, T, s.node_id_base, pods4 + p0, s.d_plan_pcol + p0, np, s.d_plan_cols, ncol, W, PC,
+                    s.d_plan_nodekey, s.d_plan_tilekey, s.d_keys + p0, s.d_victims + p0);
+            }
+            h->launches += sg.mode != 0 ? 2 : 1;
+        }
         KGPU_CUDA(h, cudaGetLastError());
     }
     KGPU_CUDA(h, cudaEventRecord(s.ev1, s.stream));
@@ -1223,7 +1256,7 @@ int kgpu_preempt_plan(kgpu_t *h, const int32_t *pods, const int32_t *lvl, int64_
     KGPU_CUDA(h, s.d_plan_pcol.reserve(P, cap));
     KGPU_CUDA(h, cudaMemcpyAsync(s.d_pods, pods, (size_t)P * 16, cudaMemcpyHostToDevice, s.stream));
     KGPU_CUDA(h, cudaMemcpyAsync(s.d_plan_pcol, pcol.data(), (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
-    return plan_launch(h, s, P, cols, false, out_keys, out_victims);
+    return plan_launch(h, s, P, cols, false, kgpu::place_segments(nullptr, nullptr, P), out_keys, out_victims);
 }
 
 int kgpu_preempt_plan_gang(kgpu_t *h, const int32_t *pods, const int32_t *lvl, const int32_t *gang, int64_t P,
@@ -1252,7 +1285,41 @@ int kgpu_preempt_plan_gang(kgpu_t *h, const int32_t *pods, const int32_t *lvl, c
     KGPU_CUDA(h, cudaMemcpyAsync(s.d_pods, pods, (size_t)P * 16, cudaMemcpyHostToDevice, s.stream));
     KGPU_CUDA(h, cudaMemcpyAsync(s.d_plan_pcol, pcol.data(), (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
     KGPU_CUDA(h, cudaMemcpyAsync(s.d_gang, gang, (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
-    return plan_launch(h, s, P, cols, true, out_keys, out_victims);
+    return plan_launch(h, s, P, cols, true, kgpu::place_segments(gang, nullptr, P), out_keys, out_victims);
+}
+
+int kgpu_preempt_plan_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *lvl, const int32_t *gang,
+                                  const int32_t *gang_domain, int64_t P, uint64_t *out_keys, uint32_t *out_victims) {
+    const char *fn = "kgpu_preempt_plan_gang_domain";
+    if (!h) return fail(h, KGPU_ERR_INVALID, "%s: NULL handle", fn);
+    std::lock_guard<std::mutex> g(h->mu);
+    if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "%s: needs a single-device handle", fn);
+    if (P < 0 || (P > 0 && (!pods || !lvl || !out_keys || !out_victims))) return fail(h, KGPU_ERR_INVALID, "%s: bad arguments", fn);
+    if (P == 0) return KGPU_OK;
+    int rc = gang ? check_gang_runs(h, fn, gang, P) : KGPU_OK;
+    if (rc != KGPU_OK) return rc;
+    if (gang_domain) {
+        rc = check_gang_domain(h, fn, gang, gang_domain, P);
+        if (rc != KGPU_OK) return rc;
+    }
+    std::vector<int4> cols;
+    std::vector<int32_t> pcol;
+    rc = plan_columns(h, fn, pods, lvl, P, cols, pcol);
+    if (rc != KGPU_OK) return rc;
+    kgpu_shard &s = h->shards[0];
+    rc = reserve_pods(h, s, P);
+    if (rc != KGPU_OK) return rc;
+    const int64_t cap = pod_headroom(P);
+    KGPU_CUDA(h, s.d_victims.reserve(P, cap));
+    KGPU_CUDA(h, s.d_plan_pcol.reserve(P, cap));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_pods, pods, (size_t)P * 16, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_plan_pcol, pcol.data(), (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
+    if (gang) {
+        KGPU_CUDA(h, s.d_gang.reserve(P, cap));
+        KGPU_CUDA(h, s.d_plan_pre.reserve(P, cap));
+        KGPU_CUDA(h, cudaMemcpyAsync(s.d_gang, gang, (size_t)P * 4, cudaMemcpyHostToDevice, s.stream));
+    }
+    return plan_launch(h, s, P, cols, gang != nullptr, kgpu::place_segments(gang, gang_domain, P), out_keys, out_victims);
 }
 
 int kgpu_get_free_masks(kgpu_t *h, int32_t *out_free_mask, int64_t n) {

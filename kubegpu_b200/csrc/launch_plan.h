@@ -47,7 +47,9 @@ inline bool place_views(const int32_t *pods, int64_t P, PlaceViews &views) {
 // kgpu_place_batch_gang_domain: the batch cut into segments, in order.  A constrained gang (a run of consecutive pods with
 // the same nonzero gang id and a nonzero gang_domain, which the host has checked its members agree on) is one domain
 // step, mode = its gang_domain: domain_trial + domain_commit.  Every maximal pod range without one is one place_sequential
-// launch on pods + begin, mode = 0.  gang_domain == nullptr (or all 0): one segment, the whole batch.
+// launch on pods + begin, mode = 0.  gang_domain == nullptr (or all 0): one segment, the whole batch.  Preemption plans
+// (kgpu_preempt_plan_gang_domain) are cut the same way: plan_sequential / gang_plan_sequential per plain range,
+// domain_plan_trial + domain_plan_commit per constrained gang.
 struct PlaceSegment {
     int64_t begin, end;
     int32_t mode;

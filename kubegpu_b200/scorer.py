@@ -218,19 +218,31 @@ class Scorer:
                                                victims.ctypes.data))
         return keys, victims
 
-    def preempt_plan(self, pods, lvl, gang=None):
+    def preempt_plan(self, pods, lvl, gang=None, gang_domain=None):
         """(keys uint64[P], victims uint32[P]) as preempt_batch, but conflict-free: pods are taken in order, each on the
         state the pods before it leave (their GPUs taken, their victims' GPUs free, neither evictable again).  Victim
         sets are disjoint.  Dry run: the handle's masks and holder table are untouched.  Pass pods in priority order.
         gang: int32[P] gang ids as for place_batch.  A gang's members evict and take all together or not at all: if a
         member misses, the members before it are undone (their victims are running pods again for later pods) and the
-        whole gang gets NO_FIT and victims 0.  An id in two separate runs raises KgpuError (ERR_INVALID)."""
+        whole gang gets NO_FIT and victims 0.  An id in two separate runs raises KgpuError (ERR_INVALID).
+        gang_domain: int32[P] as for place_batch.  A REQUIRED gang evicts and takes its GPUs inside the one domain of
+        upload_domains whose trial plan is best in (max victim level, victim count, summed cost, domain id), or gets
+        NO_FIT; a PREFERRED gang falls back to the plain gang plan (include/kgpu.h has the definition)."""
         pods, lvl = _i32(pods), _i32(lvl)
         P = pods.size // 4
         if lvl.size != P:
             raise ValueError("lvl must hold one level per pod")
         keys = np.empty(P, dtype=np.uint64)
         victims = np.empty(P, dtype=np.uint32)
+        if gang_domain is not None:
+            gang = None if gang is None else _i32(gang)
+            gang_domain = _i32(gang_domain)
+            if (gang is not None and gang.size != P) or gang_domain.size != P:
+                raise ValueError("gang and gang_domain must hold one value per pod")
+            self._check(self._L.kgpu_preempt_plan_gang_domain(self._h, pods.ctypes.data, lvl.ctypes.data,
+                                                              None if gang is None else gang.ctypes.data,
+                                                              gang_domain.ctypes.data, P, keys.ctypes.data, victims.ctypes.data))
+            return keys, victims
         if gang is None:
             self._check(self._L.kgpu_preempt_plan(self._h, pods.ctypes.data, lvl.ctypes.data, P, keys.ctypes.data,
                                                   victims.ctypes.data))
