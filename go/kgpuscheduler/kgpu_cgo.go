@@ -171,6 +171,60 @@ func (k *handle) placeBatchDomain(pods []int32, gang []int32, gangDomain []int32
 	return keys, nil
 }
 
+// uploadDomainLevels: nested network domains (kgpu_upload_domain_levels), domain[l][i] = node i's domain at level l
+// (level 0 the finest), -1 or 0..n-1; every level holds the node count, the levels nest, 1..C.KGPU_MAX_DOMAIN_LEVELS
+// levels.
+func (k *handle) uploadDomainLevels(domain [][]int32) error {
+	if len(domain) == 0 {
+		return k.uploadDomains(nil)
+	}
+	n := len(domain[0])
+	flat := make([]int32, 0, len(domain)*n)
+	for _, lv := range domain {
+		if len(lv) != n {
+			return fmt.Errorf("uploadDomainLevels: levels of different lengths")
+		}
+		flat = append(flat, lv...)
+	}
+	var d *C.int32_t
+	if len(flat) > 0 {
+		d = (*C.int32_t)(unsafe.Pointer(&flat[0]))
+	}
+	if rc := C.kgpu_upload_domain_levels(k.h, d, C.int(len(domain)), C.int64_t(n)); rc != C.KGPU_OK {
+		return k.err("kgpu_upload_domain_levels")
+	}
+	return nil
+}
+
+// placeBatchLevels: placeBatchDomain with one gang_level per pod (kgpu_place_batch_gang_levels): the highest level a
+// constrained gang may span; the gang takes the lowest level 0..gang_level with a fitting domain.  gangLevel nil is
+// placeBatchDomain.
+func (k *handle) placeBatchLevels(pods []int32, gang []int32, gangDomain []int32, gangLevel []int32, dryRun bool) ([]uint64, error) {
+	keys := make([]uint64, len(pods)/4)
+	if len(keys) == 0 {
+		return keys, nil
+	}
+	flags := C.int(0)
+	if dryRun {
+		flags = C.KGPU_PLACE_DRY_RUN
+	}
+	var g, gd, gl *C.int32_t
+	if gang != nil {
+		g = (*C.int32_t)(unsafe.Pointer(&gang[0]))
+	}
+	if gangDomain != nil {
+		gd = (*C.int32_t)(unsafe.Pointer(&gangDomain[0]))
+	}
+	if gangLevel != nil {
+		gl = (*C.int32_t)(unsafe.Pointer(&gangLevel[0]))
+	}
+	if rc := C.kgpu_place_batch_gang_levels(k.h, (*C.int32_t)(unsafe.Pointer(&pods[0])), g, gd, gl, C.int64_t(len(keys)),
+		(*C.uint64_t)(unsafe.Pointer(&keys[0])), flags); rc != C.KGPU_OK {
+		return nil, k.err("kgpu_place_batch_gang_levels")
+	}
+	return keys, nil
+}
+
 func (k *handle) freeMasks(n int64) ([]int32, error) {
 	out := make([]int32, n)
 	if n == 0 {

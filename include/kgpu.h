@@ -20,7 +20,8 @@
  *          batched over every (pod, node) pair instead of one cgo call per pair
  *   kgpu_fit_lookup / kgpu_build_fit_table / kgpu_score_pairs
  *       <- the same PodFitsDevice, called once per (node, pod) by the core: served from a host-side (node, k) table
- *   kgpu_set_free_mask[s] / kgpu_place_batch[_ex|_gang|_gang_domain] / kgpu_upload_domains / kgpu_get_free_masks
+ *   kgpu_set_free_mask[s] / kgpu_place_batch[_ex|_gang|_gang_domain|_gang_levels] / kgpu_upload_domain[s|_levels] /
+ *   kgpu_get_free_masks
  *       <- TakePodResources / ReturnPodResources       gpuschedulerplugin/gpu_scheduler.go:57-63 (no-ops there)
  *   kgpu_reduce_shards_device
  *       <- (no reference counterpart; the reference is single-process) the final
@@ -230,6 +231,48 @@ int kgpu_place_batch_gang(kgpu_t *h, const int32_t *pods, const int32_t *gang, i
 int kgpu_upload_domains(kgpu_t *h, const int32_t *domain, int64_t n);
 int kgpu_place_batch_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *gang, const int32_t *gang_domain,
                                  int64_t P, uint64_t *out_keys, int flags);
+/* Nested network domains.  Fabrics have several levels: an NVLink or leaf-switch rack inside an InfiniBand spine or
+ * scalable unit inside a pod.  A distributed job wants the smallest of them that holds it.
+ *
+ * kgpu_upload_domain_levels sets a table of `levels` (1..KGPU_MAX_DOMAIN_LEVELS) levels, domain[l * n + i] = node i's
+ * domain at level l: -1 (none) or an id 0..n-1, ids separate at each level.  Level 0 is the finest (a rack), level
+ * levels - 1 the coarsest.  The levels must nest: for a node i with domain[l][i] >= 0 and l + 1 < levels,
+ * domain[l + 1][i] >= 0, and all nodes of one level-l domain have the same level-(l + 1) domain.  A node may have no
+ * level-l domain and still have a level-(l + 1) one.  A value out of range, a nesting violation (the message names the
+ * level, the node and the two ids) or `levels` outside 1..4 is KGPU_ERR_INVALID and leaves the table unchanged.
+ * kgpu_upload_domains(h, d, n) is the one-level table.  Lifetime as for kgpu_upload_domains: before the first upload
+ * and after kgpu_upload_nodes the table has one level with every node at -1; mask and node updates leave it alone.
+ * kgpu_place_batch_gang_domain and kgpu_preempt_plan_gang_domain read level 0 and nothing else, so on a one-level table
+ * they are what they always were.
+ *
+ * kgpu_place_batch_gang_levels: kgpu_place_batch_gang_domain with gang_level[P], the highest level each constrained
+ * gang may span, 0..levels-1 (NULL = all 0).  The policy is TIGHTEST NETWORK DOMAIN FIRST, THEN GPU LINK COST.  A
+ * constrained gang with bound r is placed on the working masks F like this:
+ *   1. For l = 0, 1, ..., r: step 1 of kgpu_place_batch_gang_domain (one trial per non-empty domain) over the level-l
+ *      domains, on F.  The first level with a successful trial wins: the gang takes that level's domain with the
+ *      smallest (C_d, d), F = F_d and the members get that trial's keys.  A k = 0 member gets the domain's lowest node.
+ *   2. No domain of any level <= r fits: REQUIRED gives every member KGPU_NO_FIT and leaves F unchanged; PREFERRED
+ *      places the gang as kgpu_place_batch_gang would, over all nodes, all or nothing.
+ * Pods and gangs with gang_domain 0 are placed exactly as by kgpu_place_batch_gang.  Consequences:
+ *   Q1 gang_level NULL or all 0 is kgpu_place_batch_gang_domain, on level 0, with the same kernel launches;
+ *   Q2 kgpu_place_batch_gang_domain after a multi-level upload equals the same call after uploading level 0 alone;
+ *   Q3 with every node in level-1 domain 0, REQUIRED with r = 1 equals PREFERRED with r = 0;
+ *   Q4 the members of a placed REQUIRED gang share one domain at some level l* <= r, never -1, and for every l < l*
+ *      the gang alone with bound l gets KGPU_NO_FIT on the same state;
+ *   Q5 PREFERRED gives the REQUIRED result when that places the gang, the plain gang result otherwise;
+ *   Q6 a failed REQUIRED gang leaves F as it was.
+ * KGPU_ERR_INVALID, checked before anything runs: every check of kgpu_place_batch_gang_domain, a gang_level outside
+ * 0..levels-1 on a constrained pod, a nonzero gang_level on a pod with gang_domain 0, and members of one gang that
+ * disagree on gang_level.  Flags (KGPU_PLACE_DRY_RUN) as there.  Both calls need a single-device handle
+ * (KGPU_ERR_STATE otherwise).  Host buffers, synchronous.
+ * Cost: a constrained gang runs one trial launch per level it climbs (a launch above the winning level exits at once).
+ * A trial walks each domain with one warp.  On levels of small domains (at most 256 nodes) it reads 32 nodes per step;
+ * on levels with a larger domain it reads the minima of 32-node chunks, 32 chunks per step, built once per level by one
+ * extra launch, and rescans node by node only the chunks the trial itself has changed. */
+#define KGPU_MAX_DOMAIN_LEVELS 4
+int kgpu_upload_domain_levels(kgpu_t *h, const int32_t *domain, int levels, int64_t n);
+int kgpu_place_batch_gang_levels(kgpu_t *h, const int32_t *pods, const int32_t *gang, const int32_t *gang_domain,
+                                 const int32_t *gang_level, int64_t P, uint64_t *out_keys, int flags);
 /* Preemption (kube-scheduler's PostFilter for GPU pods): for a pod that fits nowhere, the node, GPUs and
  * lowest-priority running pods to evict.  No reference counterpart (DeviceScheduler has no preemption hook,
  * gpu_scheduler.go:21-71).  Single-device handles only (KGPU_ERR_STATE otherwise).

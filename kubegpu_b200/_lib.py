@@ -13,7 +13,7 @@ SYMBOLS = [
     "kgpu_version", "kgpu_create", "kgpu_destroy", "kgpu_last_error", "kgpu_set_weights",
     "kgpu_get_weights", "kgpu_set_variant", "kgpu_upload_nodes", "kgpu_update_node",
     "kgpu_set_free_mask", "kgpu_set_free_masks", "kgpu_remove_node", "kgpu_build_fit_table", "kgpu_fit_lookup", "kgpu_last_upload_ms", "kgpu_upload_gpu_memory", "kgpu_update_gpu_memory", "kgpu_num_nodes", "kgpu_score_batch",
-    "kgpu_score_batch_device", "kgpu_score_batch_device_ex", "kgpu_score_pairs", "kgpu_place_batch", "kgpu_place_batch_ex", "kgpu_place_batch_gang", "kgpu_upload_domains", "kgpu_place_batch_gang_domain", "kgpu_upload_holders", "kgpu_set_holders", "kgpu_preempt_batch", "kgpu_preempt_plan", "kgpu_preempt_plan_gang", "kgpu_preempt_plan_gang_domain", "kgpu_get_free_masks", "kgpu_reduce_shards_device", "kgpu_exchange_init", "kgpu_exchange_connect", "kgpu_score_batch_exchange", "kgpu_exchange_barrier", "kgpu_kernel_launches",
+    "kgpu_score_batch_device", "kgpu_score_batch_device_ex", "kgpu_score_pairs", "kgpu_place_batch", "kgpu_place_batch_ex", "kgpu_place_batch_gang", "kgpu_upload_domains", "kgpu_place_batch_gang_domain", "kgpu_upload_domain_levels", "kgpu_place_batch_gang_levels", "kgpu_upload_holders", "kgpu_set_holders", "kgpu_preempt_batch", "kgpu_preempt_plan", "kgpu_preempt_plan_gang", "kgpu_preempt_plan_gang_domain", "kgpu_get_free_masks", "kgpu_reduce_shards_device", "kgpu_exchange_init", "kgpu_exchange_connect", "kgpu_score_batch_exchange", "kgpu_exchange_barrier", "kgpu_kernel_launches",
     "kgpu_last_kernel_ms",
 ]
 
@@ -25,6 +25,7 @@ VARIANT_SPARSE = 5
 BATCH_NO_MIN_MEM = 1
 PLACE_DRY_RUN = 1
 GANG_DOMAIN_REQUIRED, GANG_DOMAIN_PREFERRED = 1, 2
+MAX_DOMAIN_LEVELS = 4
 
 _lib = None
 
@@ -95,6 +96,10 @@ def load() -> ctypes.CDLL:
     L.kgpu_upload_domains.argtypes = [vp, i32p, i64]
     L.kgpu_place_batch_gang_domain.restype = ci
     L.kgpu_place_batch_gang_domain.argtypes = [vp, vp, vp, vp, i64, vp, ci]
+    L.kgpu_upload_domain_levels.restype = ci
+    L.kgpu_upload_domain_levels.argtypes = [vp, i32p, ci, i64]
+    L.kgpu_place_batch_gang_levels.restype = ci
+    L.kgpu_place_batch_gang_levels.argtypes = [vp, vp, vp, vp, vp, i64, vp, ci]
     L.kgpu_upload_holders.restype = ci
     L.kgpu_upload_holders.argtypes = [vp, i32p, i64]
     L.kgpu_set_holders.restype = ci

@@ -84,6 +84,7 @@ const char *const GPUTopologyGeneration = "gpu/gpu-generate-topology";
 const char *const GPUMinMemoryMiB = "gpu/gpu-min-memory-mib";
 const char *const GPUGangID = "gpu/gpu-gang-id";
 const char *const GPUGangDomain = "gpu/gpu-gang-domain";
+const char *const GPUGangDomainLevel = "gpu/gpu-gang-domain-level";
 const char *const GPUPriorityLevel = "gpu/gpu-priority-level";
 
 namespace {
@@ -508,28 +509,41 @@ std::string NvidiaGPUScheduler::AddNodeFromGpusInfo(const std::string &nodeName,
 }
 
 std::string NvidiaGPUScheduler::SetNodeDomain(const std::string &nodeName, const std::string &domainName) {
+    return SetNodeDomains(nodeName, {domainName});
+}
+
+std::string NvidiaGPUScheduler::SetNodeDomains(const std::string &nodeName, const std::vector<std::string> &names) {
     auto it = nodes_.find(nodeName);
     if (it == nodes_.end()) return lastError_ = "SetNodeDomain: unknown node " + nodeName;
-    if (it->second.domain != domainName) domainsDirty_ = true;
-    it->second.domain = domainName;
+    if ((int)names.size() > KGPU_MAX_DOMAIN_LEVELS)
+        return lastError_ = "SetNodeDomains: " + std::to_string(names.size()) + " levels, at most " + std::to_string(KGPU_MAX_DOMAIN_LEVELS);
+    if (it->second.domains != names) domainsDirty_ = true;
+    it->second.domains = names;
     return "";
 }
 
-// The domain table on the device, if a domain or the node array changed since the last push: names -> ids 0, 1, ... in
-// sorted order, -1 for nodes without one.
+// The domain table on the device, if a domain or the node array changed since the last push: per level, names -> ids
+// 0, 1, ... in sorted order, -1 for nodes without one; as many levels as the longest list.
 std::string NvidiaGPUScheduler::pushDomains() {
     if (!domainsDirty_) return "";
-    std::map<std::string, int32_t> ids;
-    for (const std::string &name : indexToName_)
-        if (!nodes_[name].domain.empty()) ids.emplace(nodes_[name].domain, 0);
-    int32_t next = 0;
-    for (auto &kv : ids) kv.second = next++;
-    std::vector<int32_t> domain(indexToName_.size(), -1);
-    for (size_t i = 0; i < indexToName_.size(); i++) {
-        const std::string &d = nodes_[indexToName_[i]].domain;
-        if (!d.empty()) domain[i] = ids[d];
+    const size_t n = indexToName_.size();
+    size_t levels = 1;
+    for (const std::string &name : indexToName_) levels = std::max(levels, nodes_[name].domains.size());
+    std::vector<int32_t> domain(levels * n, -1);
+    for (size_t l = 0; l < levels; l++) {
+        std::map<std::string, int32_t> ids;
+        for (const std::string &name : indexToName_) {
+            const std::vector<std::string> &d = nodes_[name].domains;
+            if (l < d.size() && !d[l].empty()) ids.emplace(d[l], 0);
+        }
+        int32_t next = 0;
+        for (auto &kv : ids) kv.second = next++;
+        for (size_t i = 0; i < n; i++) {
+            const std::vector<std::string> &d = nodes_[indexToName_[i]].domains;
+            if (l < d.size() && !d[l].empty()) domain[l * n + i] = ids[d[l]];
+        }
     }
-    if (kgpu_upload_domains(handle_, domain.data(), (int64_t)domain.size()) != KGPU_OK) return lastError_ = kgpu_last_error(handle_);
+    if (kgpu_upload_domain_levels(handle_, domain.data(), (int)levels, (int64_t)n) != KGPU_OK) return lastError_ = kgpu_last_error(handle_);
     domainsDirty_ = false;
     return "";
 }
@@ -671,13 +685,22 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     // ids are renumbered 1, 2, ... in order of first appearance (no truncation can merge two gangs) and each member
     // moves up to its gang's first member.  order[i] = the caller's index of the pod at device position i.
     std::vector<size_t> order(P);
-    std::vector<int32_t> gang, gangDomain;          // gangDomain: in device order, empty when no pod asks for a domain
+    std::vector<int32_t> gang, gangDomain, gangLevel;   // in device order, empty when no pod asks for a domain / level
     for (size_t p = 0; p < P; p++) order[p] = p;
     const bool placing = mode == BatchMode::Sequential || mode == BatchMode::DryRun;
     if (placing || mode == BatchMode::PreemptGangDomainPlan) {
-        std::map<int64_t, int64_t> domainOfGang;
+        std::map<int64_t, int64_t> domainOfGang, levelOfGang;
         for (size_t p = 0; p < P; p++) {
             const int64_t gd = getOr0(pods[p]->Requests, GPUGangDomain), id = getOr0(pods[p]->Requests, GPUGangID);
+            const int64_t gl = getOr0(pods[p]->Requests, GPUGangDomainLevel);
+            if (gl != 0 && mode == BatchMode::PreemptGangDomainPlan)
+                return lastError_ = "pod " + pods[p]->Name + ": " + GPUGangDomainLevel + " is not supported in preemption plans (level 0 only)";
+            if (gl != 0 && gd == 0) return lastError_ = "pod " + pods[p]->Name + ": " + GPUGangDomainLevel + " without " + GPUGangDomain;
+            if (gl < 0 || gl >= KGPU_MAX_DOMAIN_LEVELS)
+                return lastError_ = "pod " + pods[p]->Name + ": " + GPUGangDomainLevel + " must be 0.." + std::to_string(KGPU_MAX_DOMAIN_LEVELS - 1);
+            if (id != 0 && !levelOfGang.emplace(id, gl).second && levelOfGang[id] != gl)
+                return lastError_ = "pod " + pods[p]->Name + ": the members of gang " + std::to_string(id) + " disagree on " + GPUGangDomainLevel;
+            if (gl != 0) gangLevel.assign(P, 0);
             if (gd != 0 && gd != KGPU_GANG_DOMAIN_REQUIRED && gd != KGPU_GANG_DOMAIN_PREFERRED)
                 return lastError_ = "pod " + pods[p]->Name + ": " + GPUGangDomain + " must be 1 (required) or 2 (preferred)";
             if (gd != 0 && id == 0) return lastError_ = "pod " + pods[p]->Name + ": " + GPUGangDomain + " without " + GPUGangID;
@@ -723,6 +746,7 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
     for (size_t i = 0; i < P; i++) {
         const size_t p = order[i];
         if (!gangDomain.empty()) gangDomain[i] = (int32_t)getOr0(pods[p]->Requests, GPUGangDomain);
+        if (!gangLevel.empty()) gangLevel[i] = (int32_t)getOr0(pods[p]->Requests, GPUGangDomainLevel);
         types::PodInfo copy = *pods[p];                    // SetGPUReqs mutates; keep the caller's pod intact
         for (auto &c : copy.InitContainers) SetGPUReqs(c.second);
         for (auto &c : copy.RunningContainers) SetGPUReqs(c.second);
@@ -751,8 +775,9 @@ std::string NvidiaGPUScheduler::runBatch(const std::vector<const types::PodInfo 
                                                        gangDomain.empty() ? nullptr : gangDomain.data(), (int64_t)P, dev.data(),
                                                        owners.data())
                    : mode == BatchMode::Snapshot ? kgpu_score_batch(handle_, req.data(), (int64_t)P, dev.data())
-                                               : kgpu_place_batch_gang_domain(handle_, req.data(), gang.empty() ? nullptr : gang.data(),
-                                                                              gangDomain.empty() ? nullptr : gangDomain.data(), (int64_t)P,
+                                               : kgpu_place_batch_gang_levels(handle_, req.data(), gang.empty() ? nullptr : gang.data(),
+                                                                              gangDomain.empty() ? nullptr : gangDomain.data(),
+                                                                              gangLevel.empty() ? nullptr : gangLevel.data(), (int64_t)P,
                                                                               dev.data(), mode == BatchMode::DryRun ? KGPU_PLACE_DRY_RUN : 0);
     if (rc != KGPU_OK) return lastError_ = kgpu_last_error(handle_);
     std::vector<uint64_t> keys(P, KGPU_NO_FIT);           // back in the caller's order

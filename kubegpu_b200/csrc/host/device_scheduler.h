@@ -98,6 +98,11 @@ extern const char *const GPUGangID;               // "gpu/gpu-gang-id"
 // no constraint.  Only on gang members, the same for every member of a gang; honoured by PlaceBatch and ProposeBatch
 // (kgpu_place_batch_gang_domain).
 extern const char *const GPUGangDomain;           // "gpu/gpu-gang-domain"
+// Extension: pod-level request "my gang may span up to this level of nested domains" (SetNodeDomains: 0 = the finest
+// level, e.g. a rack), default 0.  Only with GPUGangDomain, the same for every member of a gang; the gang takes the
+// lowest level 0..this one with a domain that fits (kgpu_place_batch_gang_levels).  PlaceBatch and ProposeBatch honour
+// it; PlanGangDomainPreemption refuses a nonzero value.
+extern const char *const GPUGangDomainLevel;      // "gpu/gpu-gang-domain-level"
 // Extension: pod-level request "my priority level", 0..15 (values outside are clamped), default 0.  PreemptBatch lets a
 // pod evict running pods of a LOWER level; every placement records the level of its pod.
 extern const char *const GPUPriorityLevel;        // "gpu/gpu-priority-level"
@@ -183,6 +188,11 @@ public:
     // "" = none, the default.  Names map to dense ids in sorted order; the device table is re-uploaded before the next
     // PlaceBatch / ProposeBatch when a domain or the node array has changed.
     std::string SetNodeDomain(const std::string &nodeName, const std::string &domainName);
+    // Nested network domains: names[l] is the node's domain at level l (0 = the finest, e.g. a rack inside a spine at
+    // level 1), "" = none at that level.  Names map to dense ids per level in sorted order; the table has as many levels
+    // as the longest list, and the levels must nest (kgpu_upload_domain_levels, checked at the next PlaceBatch).
+    // SetNodeDomain(node, name) is SetNodeDomains(node, {name}).
+    std::string SetNodeDomains(const std::string &nodeName, const std::vector<std::string> &names);
     // Node from the node agent's GPU inventory JSON (nvgputypes.GpusInfo): names exactly as the
     // agent would advertise them, then AddNode, then the REAL link matrix (not the one implied by
     // the two group levels).  Fills *nodeInfo like the agent's UpdateNodeInfo.  "" or error text.
@@ -250,7 +260,7 @@ public:
         bool explicitTopo = false;
         bool removed = false;
         std::vector<std::string> owners;      // holder-table owner o -> pod name, as last pushed to the device
-        std::string domain;                   // SetNodeDomain ("" = none)
+        std::vector<std::string> domains;     // SetNodeDomains: per level, "" = none
     };
     const NodeRecord *node(const std::string &nodeName) const;
     static int64_t PodGPUCount(const types::PodInfo &podInfo);     // k of gpu.go:295-303

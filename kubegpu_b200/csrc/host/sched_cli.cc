@@ -10,8 +10,9 @@
 //   addnode NAME KUBEALLOC [key=val ...]        AddNode with Allocatable = {key: val}
 //   rmnode NAME                                 RemoveNode
 //   topo NAME v0 .. v63                         SetNodeTopology (extension)
-//   domain NODE [NAME]                          SetNodeDomain (extension): the node's network domain, none without NAME
-//   pod NAME [topogen=V] [minmem=MiB] [gang=ID] [gangdomain=required|preferred] [priority=L]
+//   domain NODE [NAME0 [NAME1 ...]]             SetNodeDomains (extension): the node's network domain per level (level 0
+//                                               the finest), none without a NAME; "-" = none at that level
+//   pod NAME [topogen=V] [minmem=MiB] [gang=ID] [gangdomain=required|preferred] [gangdomainlevel=R] [priority=L]
 //       {run|init CNAME req=N [kube=N] [dev:key=val ...]}...
 //   fits NODE POD                               PodFitsDevice  -> fits/score + rewritten requests
 //   allocate NODE POD                           PodAllocate    -> error text + AllocateFrom
@@ -133,9 +134,11 @@ int main(int argc, char **argv) {
             printf("  err=%s\n", sched.SetNodeTopology(name, t).c_str());
         } else if (cmd == "domain") {
             std::string name, dom;
+            std::vector<std::string> names;
             in >> name;
-            in >> dom;
-            printf("  err=%s\n", sched.SetNodeDomain(name, dom).c_str());
+            while (in >> dom) names.push_back(dom == "-" ? "" : dom);
+            printf("  err=%s\n", names.size() <= 1 ? sched.SetNodeDomain(name, names.empty() ? "" : names[0]).c_str()
+                                                  : sched.SetNodeDomains(name, names).c_str());
         } else if (cmd == "pod") {
             std::string name, tok, k;
             long long v = 0;
@@ -160,6 +163,8 @@ int main(int argc, char **argv) {
                     pod.Requests[GPUGangDomain] = gd == "required" ? 1
                                                   : gd == "preferred" ? 2
                                                                       : atoll(gd.c_str());
+                } else if (tok.compare(0, 16, "gangdomainlevel=") == 0) {
+                    pod.Requests[GPUGangDomainLevel] = atoll(tok.c_str() + 16);
                 } else if (tok.compare(0, 9, "priority=") == 0) {
                     pod.Requests[GPUPriorityLevel] = atoll(tok.c_str() + 9);
                 } else if (cur && tok.compare(0, 4, "req=") == 0) {

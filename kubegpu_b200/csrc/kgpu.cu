@@ -84,12 +84,19 @@ struct kgpu_shard {
     kgpu::DeviceBuffer<unsigned long long> d_plan_nodekey;   //   per-column node keys [cols][Npad]
     kgpu::DeviceBuffer<unsigned long long> d_plan_tilekey;   //   and their tile minima [cols][T]
     kgpu::DeviceBuffer<int4> d_plan_pre;       // kgpu_preempt_plan_gang: each placed member's pre-image {F, H row} [P]
-    kgpu::DeviceBuffer<int32_t> d_dom_off;     // kgpu_upload_domains: [D + 1] each domain's range of d_dom_nodes,
-    kgpu::DeviceBuffer<int32_t> d_dom_nodes;   //   its nodes in increasing index (nodes of no domain left out)
-    int32_t n_dom = 0;               // D; 0 = every node in no domain (no upload since the last kgpu_upload_nodes)
+    kgpu::DeviceBuffer<int32_t> d_dom_off;     // kgpu_upload_domain_levels (launch_plan.h: domain_table): each level's
+    kgpu::DeviceBuffer<int32_t> d_dom_nodes;   //   [D_l + 1] domain ranges of d_dom_nodes, level 0 first
+    int32_t n_dom = 0;               // D_0; 0 = no node in a level-0 domain (so after kgpu_upload_nodes)
+    std::vector<kgpu::DomainLevel> dom_levels = {{0, 0}};   // each level's D_l and base in d_dom_off, its chunks
+    kgpu::DeviceBuffer<int32_t> d_dom_chunk;   // the chunked walk: each domain's chunk range (laid out as d_dom_off),
+    kgpu::DeviceBuffer<int32_t> d_chunk_begin; //   each chunk's first entry of d_dom_nodes [chunks + 1],
+    int64_t n_chunks = 0;
+    kgpu::DeviceBuffer<unsigned long long> d_dom_cmin;   //   per call: the chunk minima [views * 9][chunks],
+    kgpu::DeviceBuffer<uint32_t> d_dom_cstamp;           //   each chunk's trial stamp [chunks]
+    kgpu::DeviceBuffer<int32_t> d_dom_pairs;             //   and each chunked trial's (view, k) pairs
     kgpu::DeviceBuffer<int32_t> d_dom_mask;    // domain steps: per-node working mask of the trials [n]
     kgpu::DeviceBuffer<uint32_t> d_dom_stamp;  //   and the stamp of the trial that wrote it [n]
-    kgpu::DeviceBuffer<unsigned long long> d_dom_best;   //   per step: (C_d << 32 | d) of the best trial
+    kgpu::DeviceBuffer<unsigned long long> d_dom_best;   //   per (step, level): (C_d << 32 | d) of the best trial
     kgpu::DeviceBuffer<uint2> d_dom_hold;      // plan domain steps: per-node working holder row of the trials [n]
     kgpu::DeviceBuffer<unsigned long long> d_dom_score;  //   and each domain's trial score [D]
     int64_t class_count[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -621,6 +628,8 @@ int upload_nodes(kgpu_ctx *h, const int32_t *topo, const int32_t *free_mask, int
         s.n = cnt;
         s.has_hold = false;            // a new node array has no holders
         s.n_dom = 0;                   // and no domains
+        s.dom_levels = {{0, 0}};
+        s.n_chunks = 0;
         s.node_id_base = node_id_base + off;
         s.order_dirty = true;
         s.compact_dirty = true;
@@ -861,29 +870,80 @@ int check_gang_domain(kgpu_ctx *h, const char *fn, const int32_t *gang, const in
 }
 }  // namespace
 
-int kgpu_upload_domains(kgpu_t *h, const int32_t *domain, int64_t n) {
-    if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_domains: NULL handle");
+namespace {
+// kgpu_upload_domains is the one-level case, with its own name and messages (flat: domain[i] rather than domain[l][i]).
+int upload_domain_levels(kgpu_ctx *h, const char *fn, bool flat, const int32_t *domain, int levels, int64_t n) {
+    if (!h) return fail(h, KGPU_ERR_INVALID, "%s: NULL handle", fn);
     std::lock_guard<std::mutex> g(h->mu);
-    if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_upload_domains: needs a single-device handle");
-    if (n != h->n_total || (n > 0 && !domain)) return fail(h, KGPU_ERR_INVALID, "kgpu_upload_domains: n must equal kgpu_num_nodes");
-    std::vector<int32_t> off, nodes;
-    const int64_t bad = kgpu::domain_lists(domain, n, off, nodes);
-    if (bad >= 0)
-        return fail(h, KGPU_ERR_INVALID, "kgpu_upload_domains: domain[%lld] = %d is neither -1 nor 0..%lld", (long long)bad, domain[bad],
+    if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "%s: needs a single-device handle", fn);
+    if (levels < 1 || levels > KGPU_MAX_DOMAIN_LEVELS)
+        return fail(h, KGPU_ERR_INVALID, "%s: levels = %d is outside 1..%d", fn, levels, KGPU_MAX_DOMAIN_LEVELS);
+    if (n != h->n_total || (n > 0 && !domain)) return fail(h, KGPU_ERR_INVALID, "%s: n must equal kgpu_num_nodes", fn);
+    kgpu::DomainTable t;
+    const kgpu::DomainTableError e = kgpu::domain_table(domain, levels, n, t);
+    switch (e.kind) {
+    case kgpu::DomainTableError::none: break;
+    case kgpu::DomainTableError::out_of_range:
+        if (flat)
+            return fail(h, KGPU_ERR_INVALID, "%s: domain[%lld] = %d is neither -1 nor 0..%lld", fn, (long long)e.node, e.id,
+                        (long long)(n - 1));
+        return fail(h, KGPU_ERR_INVALID, "%s: domain[%d][%lld] = %d is neither -1 nor 0..%lld", fn, e.level, (long long)e.node, e.id,
                     (long long)(n - 1));
+    case kgpu::DomainTableError::no_parent:
+        return fail(h, KGPU_ERR_INVALID, "%s: level %d: node %lld is in domain %d but in no level-%d domain (-1)", fn, e.level,
+                    (long long)e.node, e.id, e.level + 1);
+    case kgpu::DomainTableError::split:
+        return fail(h, KGPU_ERR_INVALID, "%s: level %d: domain %d is not nested: node %lld is in level-%d domain %d, node %lld in %d",
+                    fn, e.level, e.id, (long long)e.other_node, e.level + 1, e.other, (long long)e.node, e.other2);
+    }
     kgpu_shard &s = h->shards[0];
     KGPU_CUDA(h, cudaSetDevice(s.dev));
-    KGPU_CUDA(h, s.d_dom_off.reserve((int64_t)off.size()));
-    KGPU_CUDA(h, s.d_dom_nodes.reserve(std::max<int64_t>(1, (int64_t)nodes.size())));
-    KGPU_CUDA(h, cudaMemcpyAsync(s.d_dom_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice, s.stream));
-    if (!nodes.empty()) KGPU_CUDA(h, cudaMemcpyAsync(s.d_dom_nodes, nodes.data(), nodes.size() * 4, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, s.d_dom_off.reserve((int64_t)t.off.size()));
+    KGPU_CUDA(h, s.d_dom_chunk.reserve((int64_t)t.chunk.size()));
+    KGPU_CUDA(h, s.d_chunk_begin.reserve((int64_t)t.chunk_begin.size()));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_dom_chunk, t.chunk.data(), t.chunk.size() * 4, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_chunk_begin, t.chunk_begin.data(), t.chunk_begin.size() * 4, cudaMemcpyHostToDevice, s.stream));
+    KGPU_CUDA(h, s.d_dom_nodes.reserve(std::max<int64_t>(1, (int64_t)t.nodes.size())));
+    KGPU_CUDA(h, cudaMemcpyAsync(s.d_dom_off, t.off.data(), t.off.size() * 4, cudaMemcpyHostToDevice, s.stream));
+    if (!t.nodes.empty()) KGPU_CUDA(h, cudaMemcpyAsync(s.d_dom_nodes, t.nodes.data(), t.nodes.size() * 4, cudaMemcpyHostToDevice, s.stream));
     KGPU_CUDA(h, cudaStreamSynchronize(s.stream));
-    s.n_dom = (int32_t)(off.size() - 1);
+    s.n_dom = t.level[0].D;
+    s.dom_levels = t.level;
+    s.n_chunks = (int64_t)t.chunk_begin.size() - 1;
+    return KGPU_OK;
+}
+}  // namespace
+
+int kgpu_upload_domains(kgpu_t *h, const int32_t *domain, int64_t n) {
+    return upload_domain_levels(h, "kgpu_upload_domains", true, domain, 1, n);
+}
+
+int kgpu_upload_domain_levels(kgpu_t *h, const int32_t *domain, int levels, int64_t n) {
+    return upload_domain_levels(h, "kgpu_upload_domain_levels", false, domain, levels, n);
+}
+
+namespace {
+// gang_level: within 0..levels-1 on constrained pods, 0 on the others, the same for all members of a gang.
+int check_gang_level(kgpu_ctx *h, const char *fn, const int32_t *gang, const int32_t *gang_domain, const int32_t *gang_level,
+                     int64_t P, int levels) {
+    for (int64_t p = 0; p < P; p++) {
+        const int32_t r = gang_level[p];
+        if ((gang_domain == nullptr || gang_domain[p] == 0) && r != 0)
+            return fail(h, KGPU_ERR_INVALID, "%s: gang_level[%lld] = %d on a pod without a domain constraint", fn, (long long)p, r);
+        if (r < 0 || r >= levels)
+            return fail(h, KGPU_ERR_INVALID, "%s: gang_level[%lld] = %d is outside 0..%d (the domain table has %d level%s)", fn,
+                        (long long)p, r, levels - 1, levels, levels == 1 ? "" : "s");
+        if (gang && p > 0 && gang[p] != 0 && gang[p] == gang[p - 1] && r != gang_level[p - 1])
+            return fail(h, KGPU_ERR_INVALID, "%s: the members of gang %d disagree on gang_level (%d at pod %lld, %d at pod %lld)", fn,
+                        gang[p], gang_level[p - 1], (long long)(p - 1), r, (long long)p);
+    }
     return KGPU_OK;
 }
 
-int kgpu_place_batch_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *gang, const int32_t *gang_domain, int64_t P,
-                                 uint64_t *out_keys, int flags) {
+// kgpu_place_batch_gang_levels under the name fn: kgpu_place_batch_gang_domain is gang_level == NULL, and its messages
+// keep the names they have always had.
+int place_batch_levels(kgpu_t *h, const char *fn, const int32_t *pods, const int32_t *gang, const int32_t *gang_domain,
+                       const int32_t *gang_level, int64_t P, uint64_t *out_keys, int flags) {
     if (!h) return fail(h, KGPU_ERR_INVALID, "kgpu_place_batch: NULL handle");
     std::lock_guard<std::mutex> g(h->mu);
     if (h->shards.size() != 1) return fail(h, KGPU_ERR_STATE, "kgpu_place_batch: needs a single-device handle");
@@ -894,7 +954,11 @@ int kgpu_place_batch_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *
         if (rc != KGPU_OK) return rc;
     }
     if (gang_domain) {
-        const int rc = check_gang_domain(h, "kgpu_place_batch_gang_domain", gang, gang_domain, P);
+        const int rc = check_gang_domain(h, fn, gang, gang_domain, P);
+        if (rc != KGPU_OK) return rc;
+    }
+    if (gang_level) {
+        const int rc = check_gang_level(h, fn, gang, gang_domain, gang_level, P, (int)h->shards[0].dom_levels.size());
         if (rc != KGPU_OK) return rc;
     }
     kgpu::PlaceViews views;
@@ -934,30 +998,66 @@ int kgpu_place_batch_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *
             KGPU_CUDA(h, cudaFuncSetAttribute(kgpu::place_sequential<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kgpu::PLACE_DYN_SMEM));
             s.place_attr_done = true;
         }
-        const std::vector<kgpu::PlaceSegment> segs = kgpu::place_segments(gang, gang_domain, P);
-        const int64_t steps = std::count_if(segs.begin(), segs.end(), [](const kgpu::PlaceSegment &sg) { return sg.mode != 0; });
+        const std::vector<kgpu::PlaceSegment> segs = kgpu::place_segments(gang, gang_domain, P, gang_level);
+        int64_t trials = 0;            // one best[] entry and one stamp per (step, level), one stamp per commit
+        std::vector<int32_t> pairs;    // the (view, k) pairs of every step that climbs to a chunked level, step after step
+        std::vector<int64_t> pair_at;
+        for (const kgpu::PlaceSegment &sg : segs) {
+            if (sg.mode == 0) continue;
+            trials += sg.level + 1;
+            pair_at.push_back((int64_t)pairs.size());
+            bool chunked = false;
+            for (int32_t l = 0; l <= sg.level; l++) chunked = chunked || kgpu::domain_level_chunked(s.dom_levels[(size_t)l]);
+            if (chunked) kgpu::domain_pairs(pods, sg.begin, sg.end, views, pairs);
+        }
+        pair_at.push_back((int64_t)pairs.size());
         kgpu::DomainArgs da = {};
-        if (steps > 0) {               // the trials' scratch: stamps 2 i + 1 (trials of step i) and 2 i + 2 (its commit)
+        if (trials > 0) {
             KGPU_CUDA(h, s.d_dom_mask.reserve(s.n));
             KGPU_CUDA(h, s.d_dom_stamp.reserve(s.n));
-            KGPU_CUDA(h, s.d_dom_best.reserve(steps, pod_headroom(steps)));
-            if (s.n_dom == 0) KGPU_CUDA(h, s.d_dom_off.reserve(1));
+            KGPU_CUDA(h, s.d_dom_best.reserve(trials, pod_headroom(trials)));
+            KGPU_CUDA(h, s.d_dom_off.reserve(1));
             KGPU_CUDA(h, cudaMemsetAsync(s.d_dom_stamp, 0, (size_t)s.n * 4, s.stream));
-            KGPU_CUDA(h, cudaMemsetAsync(s.d_dom_best, 0xFF, (size_t)steps * 8, s.stream));
+            KGPU_CUDA(h, cudaMemsetAsync(s.d_dom_best, 0xFF, (size_t)trials * 8, s.stream));
             da = kgpu::DomainArgs{d_free, s.d_mem, Npad, T, s.node_id_base, views, s.d_nodebest, s.d_tilebest, s.d_half,
                                   s.d_dom_off, s.d_dom_nodes, s.d_dom_mask, s.d_dom_stamp};
+            if (!pairs.empty()) {
+                KGPU_CUDA(h, s.d_dom_cmin.reserve(views.n * 9 * s.n_chunks));
+                KGPU_CUDA(h, s.d_dom_cstamp.reserve(s.n_chunks));
+                KGPU_CUDA(h, s.d_dom_pairs.reserve((int64_t)pairs.size(), pod_headroom((int64_t)pairs.size())));
+                KGPU_CUDA(h, cudaMemsetAsync(s.d_dom_cstamp, 0, (size_t)s.n_chunks * 4, s.stream));
+                KGPU_CUDA(h, cudaMemcpyAsync(s.d_dom_pairs, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, s.stream));
+                da.dom_chunk = s.d_dom_chunk, da.chunk_begin = s.d_chunk_begin, da.cmin = s.d_dom_cmin, da.cstamp = s.d_dom_cstamp;
+                da.chunks = s.n_chunks;
+            }
         }
         const int4 *pods4 = reinterpret_cast<const int4 *>(s.d_pods.get());
-        int64_t step = 0;
+        int64_t slot = 0, step = 0;
+        uint32_t stamp = 0;
         for (const kgpu::PlaceSegment &sg : segs) {
             const int64_t p0 = sg.begin, np = sg.end - sg.begin;
             if (sg.mode != 0) {
-                const uint32_t stamp = (uint32_t)(2 * step + 1);
-                kgpu::domain_trial<<<kgpu::domain_trial_blocks(s.n_dom, (int64_t)s.sm_count * 8), kgpu::DOM_THREADS, 0, s.stream>>>(
-                    da, pods4 + p0, np, s.n_dom, stamp, s.d_dom_best + step);
-                kgpu::domain_commit<<<1, kgpu::DOM_COMMIT_THREADS, 0, s.stream>>>(da, pods4 + p0, np, sg.mode, stamp + 1,
-                                                                                 s.d_dom_best + step, s.d_keys + p0);
+                int32_t chunked_levels = 0;
+                const int64_t npair = pair_at[(size_t)step + 1] - pair_at[(size_t)step];
+                for (int32_t l = 0; l <= sg.level; l++) {
+                    const kgpu::DomainLevel lv = s.dom_levels[(size_t)l];
+                    const bool chunked = kgpu::domain_level_chunked(lv) && npair > 0;
+                    if (chunked) {
+                        kgpu::domain_chunk_min<<<dim3(kgpu::domain_trial_blocks(lv.C, (int64_t)s.sm_count * 8), (unsigned)npair),
+                                                 kgpu::DOM_THREADS, 0, s.stream>>>(da, lv.chunk0, lv.C, s.d_dom_pairs + pair_at[(size_t)step],
+                                                                                   s.d_dom_best + slot, l);
+                        h->launches++;
+                    }
+                    chunked_levels |= chunked ? 1 << l : 0;
+                    kgpu::domain_trial<<<kgpu::domain_trial_blocks(lv.D, (int64_t)s.sm_count * 8), kgpu::DOM_THREADS, 0, s.stream>>>(
+                        da, pods4 + p0, np, lv.D, ++stamp, s.d_dom_best + slot, l, lv.base, chunked ? 1 : 0);
+                }
+                kgpu::domain_commit<<<1, kgpu::DOM_COMMIT_THREADS, 0, s.stream>>>(da, pods4 + p0, np, sg.mode, ++stamp,
+                                                                                 s.d_dom_best + slot, s.d_keys + p0, sg.level + 1,
+                                                                                 chunked_levels);
+                slot += sg.level + 1;
                 step++;
+                h->launches += sg.level + 1;
             } else if (gang) {
                 kgpu::place_sequential<true><<<1, kgpu::PLACE_THREADS, kgpu::PLACE_DYN_SMEM, s.stream>>>(
                     s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base, pods4 + p0, np, W, views, s.d_nodebest, s.d_tilebest, T,
@@ -967,7 +1067,7 @@ int kgpu_place_batch_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *
                     s.d_topo, d_free, s.d_mem, s.n, Npad, s.node_id_base, pods4 + p0, np, W, views, s.d_nodebest, s.d_tilebest, T,
                     s.d_half, s.d_keys + p0);
             }
-            h->launches += sg.mode != 0 ? 2 : 1;
+            h->launches++;
         }
         if (!dry) {
             s.order_dirty = true;        // the free masks have changed on the device: re-sort + recompact lazily
@@ -984,6 +1084,17 @@ int kgpu_place_batch_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *
         h->last_kernel_ms = ms;
     }
     return KGPU_OK;
+}
+}  // namespace
+
+int kgpu_place_batch_gang_domain(kgpu_t *h, const int32_t *pods, const int32_t *gang, const int32_t *gang_domain, int64_t P,
+                                 uint64_t *out_keys, int flags) {
+    return place_batch_levels(h, "kgpu_place_batch_gang_domain", pods, gang, gang_domain, nullptr, P, out_keys, flags);
+}
+
+int kgpu_place_batch_gang_levels(kgpu_t *h, const int32_t *pods, const int32_t *gang, const int32_t *gang_domain,
+                                 const int32_t *gang_level, int64_t P, uint64_t *out_keys, int flags) {
+    return place_batch_levels(h, "kgpu_place_batch_gang_levels", pods, gang, gang_domain, gang_level, P, out_keys, flags);
 }
 
 namespace {

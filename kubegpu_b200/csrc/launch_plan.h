@@ -44,17 +44,19 @@ inline bool place_views(const int32_t *pods, int64_t P, PlaceViews &views) {
     return true;
 }
 
-// kgpu_place_batch_gang_domain: the batch cut into segments, in order.  A constrained gang (a run of consecutive pods with
+// kgpu_place_batch_gang_levels: the batch cut into segments, in order.  A constrained gang (a run of consecutive pods with
 // the same nonzero gang id and a nonzero gang_domain, which the host has checked its members agree on) is one domain
-// step, mode = its gang_domain: domain_trial + domain_commit.  Every maximal pod range without one is one place_sequential
-// launch on pods + begin, mode = 0.  gang_domain == nullptr (or all 0): one segment, the whole batch.  Preemption plans
-// (kgpu_preempt_plan_gang_domain) are cut the same way: plan_sequential / gang_plan_sequential per plain range,
-// domain_plan_trial + domain_plan_commit per constrained gang.
+// step, mode = its gang_domain, level = its gang_level (0 without gang_level): one domain_trial per level 0..level, then
+// domain_commit.  Every maximal pod range without one is one place_sequential launch on pods + begin, mode = 0.
+// gang_domain == nullptr (or all 0): one segment, the whole batch.  Preemption plans (kgpu_preempt_plan_gang_domain) are
+// cut the same way, without levels: plan_sequential / gang_plan_sequential per plain range, domain_plan_trial +
+// domain_plan_commit per constrained gang.
 struct PlaceSegment {
     int64_t begin, end;
-    int32_t mode;
+    int32_t mode, level;
 };
-inline std::vector<PlaceSegment> place_segments(const int32_t *gang, const int32_t *gang_domain, int64_t P) {
+inline std::vector<PlaceSegment> place_segments(const int32_t *gang, const int32_t *gang_domain, int64_t P,
+                                                const int32_t *gang_level = nullptr) {
     std::vector<PlaceSegment> seg;
     int64_t p = 0, plain = 0;
     while (p < P) {
@@ -64,11 +66,11 @@ inline std::vector<PlaceSegment> place_segments(const int32_t *gang, const int32
         }
         int64_t e = p + 1;
         while (e < P && gang[e] == gang[p]) e++;
-        if (plain < p) seg.push_back({plain, p, 0});
-        seg.push_back({p, e, gang_domain[p]});
+        if (plain < p) seg.push_back({plain, p, 0, 0});
+        seg.push_back({p, e, gang_domain[p], gang_level ? gang_level[p] : 0});
         p = plain = e;
     }
-    if (plain < P) seg.push_back({plain, P, 0});
+    if (plain < P) seg.push_back({plain, P, 0, 0});
     return seg;
 }
 
@@ -90,6 +92,104 @@ inline int64_t domain_lists(const int32_t *domain, int64_t n, std::vector<int32_
     for (int64_t i = 0; i < n; i++)
         if (domain[i] >= 0) nodes[(size_t)at[(size_t)domain[i]]++] = (int32_t)i;
     return -1;
+}
+
+// kgpu_upload_domain_levels: every level's domain_lists, one level after another in one off[] and one nodes[].  Level
+// l's D_l domains have their ranges at off[base_l .. base_l + D_l], and those ranges index the shared nodes[]; level 0
+// comes first with base 0, so off[0 .. D_0] and nodes[] read alone are level 0's domain_lists (what the level-0-only
+// callers read).  Domain d of level l is the table's domain base_l + d.  For the chunked walk every domain's list is cut
+// into chunks of DOM_CHUNK entries, numbered over the whole table in list order: chunk c is nodes[chunk_begin[c] ..
+// chunk_begin[c + 1]), domain g's chunks are chunk[g] .. chunk[g + 1] (chunk[] laid out as off[]), level l's are
+// chunk0 .. chunk0 + C - 1.  largest: the level's largest domain, which picks its walk (domain_level_chunked).
+struct DomainLevel {
+    int32_t D, base;
+    int64_t largest, chunk0, C;
+};
+struct DomainTable {
+    std::vector<int32_t> off, nodes, chunk, chunk_begin = {0};
+    std::vector<DomainLevel> level;
+};
+// Why domain_table refused an upload: kind out_of_range: domain[level][node] = id is outside -1..n-1; no_parent: node
+// is in level-`level` domain id but in no level + 1 domain (other = -1); split: level-`level` domain id has node
+// other_node in level + 1 domain other and node `node` in level + 1 domain other2.
+struct DomainTableError {
+    enum Kind { none, out_of_range, no_parent, split } kind = none;
+    int level = 0;
+    int64_t node = -1, other_node = -1;
+    int32_t id = 0, other = 0, other2 = 0;
+};
+// domain[levels][n]: builds t, or leaves it untouched and says why not.  Nesting: a node with a level-l domain has a
+// level-(l + 1) domain, the same one for every node of its level-l domain (one pass per level).
+inline DomainTableError domain_table(const int32_t *domain, int levels, int64_t n, DomainTable &t) {
+    DomainTableError err;
+    DomainTable out;
+    for (int l = 0; l < levels; l++) {
+        std::vector<int32_t> off, nodes;
+        const int32_t *dl = domain + (int64_t)l * n;
+        const int64_t bad = domain_lists(dl, n, off, nodes);
+        if (bad >= 0) {
+            err.kind = DomainTableError::out_of_range, err.level = l, err.node = bad, err.id = dl[bad];
+            return err;
+        }
+        const int32_t shift = (int32_t)out.nodes.size();
+        DomainLevel lv = {(int32_t)off.size() - 1, (int32_t)out.off.size(), 0, (int64_t)out.chunk_begin.size() - 1, 0};
+        for (size_t d = 0; d < off.size(); d++) {
+            out.off.push_back(off[d] + shift);
+            out.chunk.push_back((int32_t)out.chunk_begin.size() - 1);
+            if (d + 1 == off.size()) break;
+            lv.largest = std::max<int64_t>(lv.largest, off[d + 1] - off[d]);
+            for (int32_t e = off[d] + DOM_CHUNK; e < off[d + 1]; e += DOM_CHUNK) out.chunk_begin.push_back(e + shift);
+            if (off[d + 1] > off[d]) out.chunk_begin.push_back(off[d + 1] + shift);
+        }
+        lv.C = (int64_t)out.chunk_begin.size() - 1 - lv.chunk0;
+        out.level.push_back(lv);
+        out.nodes.insert(out.nodes.end(), nodes.begin(), nodes.end());
+    }
+    for (int l = 0; l + 1 < levels; l++) {
+        const int32_t *dl = domain + (int64_t)l * n, *up = domain + (int64_t)(l + 1) * n;
+        std::vector<int64_t> first((size_t)out.level[(size_t)l].D, -1);   // the first node seen of each level-l domain
+        for (int64_t i = 0; i < n; i++) {
+            const int32_t d = dl[i];
+            if (d < 0) continue;
+            if (up[i] < 0) {
+                err.kind = DomainTableError::no_parent, err.level = l, err.node = i, err.id = d, err.other = -1;
+                return err;
+            }
+            int64_t &f = first[(size_t)d];
+            if (f < 0) f = i;
+            else if (up[f] != up[i]) {
+                err.kind = DomainTableError::split, err.level = l, err.node = i, err.other_node = f, err.id = d;
+                err.other = up[f], err.other2 = up[i];
+                return err;
+            }
+        }
+    }
+    t = std::move(out);
+    return err;
+}
+
+// A level whose largest domain has more than DOM_CHUNKED_MIN nodes is walked by chunk minima (a domain_chunk_min launch
+// before each of its trials); smaller ones by the plain walk, whose trial is a single launch.  At racks of 8..128 nodes
+// the plain walk measures as fast as before the chunked walk existed; at spines of 1024 and more the chunked walk is
+// faster (DESIGN.md §6).  force: the chunked walk everywhere (the emulator's test seam, not a user option).
+constexpr int64_t DOM_CHUNKED_MIN = 256;
+inline bool domain_level_chunked(const DomainLevel &lv, bool force = false) {
+    return lv.C > 0 && (force || lv.largest > DOM_CHUNKED_MIN);
+}
+
+// The distinct (view, k) pairs v * 9 + k of the members pods[begin .. end) with k in 0..8, view as domain_pod_view
+// picks it: the rows domain_chunk_min builds for the step.
+inline void domain_pairs(const int32_t *pods, int64_t begin, int64_t end, const PlaceViews &views, std::vector<int32_t> &pairs) {
+    const size_t first = pairs.size();
+    for (int64_t p = begin; p < end; p++) {
+        const int32_t k = pods[4 * p];
+        if (k < 0 || k > 8) continue;
+        int v = 0;
+        for (int j = 1; j < views.n; j++)
+            if (pods[4 * p + 3] == views.min_mem[j]) v = j;
+        const int32_t pr = v * 9 + k;
+        if (std::find(pairs.begin() + (std::ptrdiff_t)first, pairs.end(), pr) == pairs.end()) pairs.push_back(pr);
+    }
 }
 
 // domain_trial's grid: warp per domain, at most max_blocks blocks (grid-strided beyond), at least one

@@ -147,7 +147,7 @@ class Scorer:
         return out
 
     def place_batch(self, pods, out: Optional[np.ndarray] = None, dry_run: bool = False, gang=None,
-                    gang_domain=None) -> np.ndarray:
+                    gang_domain=None, gang_level=None) -> np.ndarray:
         """Stateful sequential placement: pods in order, each takes its GPUs (device free masks change).
         dry_run: conflict-free proposals on a scratch copy of the masks, the handle's state is untouched.
         gang: int32[P] gang ids, 0 = the pod is on its own.  A run of consecutive pods with the same nonzero id
@@ -155,36 +155,56 @@ class Scorer:
         whole gang gets NO_FIT.  An id in two separate runs raises KgpuError (ERR_INVALID).
         gang_domain: int32[P], 0 = no constraint, 1 (GANG_DOMAIN_REQUIRED) = the gang is placed inside one domain of
         upload_domains or not at all, 2 (GANG_DOMAIN_PREFERRED) = inside one domain if one fits, else as a plain gang.
-        Nonzero only on gang members, the same for every member of a gang (include/kgpu.h has the definition)."""
+        Nonzero only on gang members, the same for every member of a gang (include/kgpu.h has the definition).
+        gang_level: int32[P], the highest level of a multi-level domain table a constrained gang may span (0 on other
+        pods, the same for every member): the gang takes the lowest level 0..gang_level with a domain that fits, then
+        the cheapest domain there.  None = all 0, which is the level-0 placement."""
         pods = _i32(pods)
         P = pods.size // 4
         if out is None:
             out = np.empty(P, dtype=np.uint64)
         flags = _lib.PLACE_DRY_RUN if dry_run else 0
-        if gang is None and gang_domain is None:
+        if gang is None and gang_domain is None and gang_level is None:
             self._check(self._L.kgpu_place_batch_ex(self._h, pods.ctypes.data, P, out.ctypes.data, flags))
             return out
         if gang is not None:
             gang = _i32(gang)
             if gang.size != P:
                 raise ValueError("gang must hold one id per pod")
-        if gang_domain is None:
+        if gang_domain is None and gang_level is None:
             self._check(self._L.kgpu_place_batch_gang(self._h, pods.ctypes.data, gang.ctypes.data, P, out.ctypes.data, flags))
             return out
-        gang_domain = _i32(gang_domain)
-        if gang_domain.size != P:
-            raise ValueError("gang_domain must hold one value per pod")
-        self._check(self._L.kgpu_place_batch_gang_domain(self._h, pods.ctypes.data, None if gang is None else gang.ctypes.data,
-                                                         gang_domain.ctypes.data, P, out.ctypes.data, flags))
+        if gang_domain is not None:
+            gang_domain = _i32(gang_domain)
+            if gang_domain.size != P:
+                raise ValueError("gang_domain must hold one value per pod")
+        g = None if gang is None else gang.ctypes.data
+        gd = None if gang_domain is None else gang_domain.ctypes.data
+        if gang_level is None:
+            self._check(self._L.kgpu_place_batch_gang_domain(self._h, pods.ctypes.data, g, gd, P,
+                                                             out.ctypes.data, flags))
+            return out
+        gang_level = _i32(gang_level)
+        if gang_level.size != P:
+            raise ValueError("gang_level must hold one value per pod")
+        self._check(self._L.kgpu_place_batch_gang_levels(self._h, pods.ctypes.data, g, gd,
+                                                         gang_level.ctypes.data, P, out.ctypes.data, flags))
         return out
 
     def upload_domains(self, domain) -> None:
         """domain[N]: each node's network domain, -1 (none) or 0..N-1 (the nodes under one leaf switch, one scalable
-        unit or one NVLink Switch domain).  Until the first upload, and after upload_nodes, every node is in none."""
+        unit or one NVLink Switch domain).  domain[L, N]: L nested levels (1..MAX_DOMAIN_LEVELS), level 0 the finest
+        (a rack), each level's ids separate; the nodes of one level-l domain share one level-(l + 1) domain
+        (kgpu_upload_domain_levels has the rules).  Until the first upload, and after upload_nodes, every node is in
+        none."""
         dom = _i32(domain)
-        if dom.size != self.num_nodes:
-            raise ValueError("domain must hold one value per node")
-        self._check(self._L.kgpu_upload_domains(self._h, dom.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), dom.size))
+        if dom.ndim not in (1, 2) or dom.shape[-1] != self.num_nodes:
+            raise ValueError("domain must hold one value per node (per level)")
+        ptr = dom.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
+        if dom.ndim == 1:
+            self._check(self._L.kgpu_upload_domains(self._h, ptr, dom.size))
+        else:
+            self._check(self._L.kgpu_upload_domain_levels(self._h, ptr, dom.shape[0], dom.shape[1]))
 
     # -- preemption (PostFilter) -----------------------------------------------------
     def upload_holders(self, holders) -> None:

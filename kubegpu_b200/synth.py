@@ -252,3 +252,24 @@ def gen_domains(N: int, size: int, seed: int = SEED_DOMAINS) -> np.ndarray:
     dom = np.empty(N, dtype=np.int32)
     dom[order] = (np.arange(N) // size).astype(np.int32)
     return dom
+
+
+def gen_domain_levels(N: int, sizes, seed: int = SEED_DOMAINS) -> np.ndarray:
+    """Nested network domains for N nodes, for example racks of 32 inside spines of 1024: int32[len(sizes), N].  The
+    nodes are laid out in a seeded permutation (so no domain is a contiguous index range) and level 0 cuts it into
+    domains of sizes[0] slots, as gen_domains(N, sizes[0], seed) does.  Level l + 1 groups whole level-l domains: each
+    goes to the one whose range of sizes[l + 1] slots holds its first slot, so its domains hold about sizes[l + 1]
+    nodes (exactly that many, but the last, when sizes[l + 1] is a multiple of sizes[l]).  Sizes must increase."""
+    sizes = [int(s) for s in sizes]
+    if not sizes or sizes[0] < 1 or any(b <= a for a, b in zip(sizes, sizes[1:])):
+        raise ValueError("sizes must be positive and increasing")
+    order = np.argsort(rand_u64(seed, 31, N), kind="stable")
+    out = np.empty((len(sizes), N), dtype=np.int32)
+    out[0, order] = (np.arange(N) // sizes[0]).astype(np.int32)
+    lead = out[0].astype(np.int64) * sizes[0]                  # each node's level-l domain's first slot
+    for lv in range(1, len(sizes)):
+        out[lv] = (lead // sizes[lv]).astype(np.int32)
+        first = np.full(int(out[lv].max()) + 1 if N else 0, np.iinfo(np.int64).max, np.int64)
+        np.minimum.at(first, out[lv], lead)
+        lead = first[out[lv]]
+    return out

@@ -7,8 +7,8 @@ nodes (synth.gen_domains) and into one domain holding every node.  Per domain si
   (c) the same pods with gang_domain = 0 (plain kgpu_place_batch_gang; the same for every domain size);
   (d) the CPU twin (tests/gang_domain_twin) of (a) on one host thread, which (a) must equal key for key.
 Device figures are dry runs on the uploaded state: the CUDA-event time of the whole device path (place_init to the last
-launch) and the wall time of the call, median of 10 with min..max (3 for the single domain: one warp walks all 100k
-nodes per member, about N / 32 dependent steps, so that line is slow by construction).  For each run: gangs placed
+launch) and the wall time of the call, median of 10 with min..max (3 for the single domain, the slowest line: one warp
+walks all 100k nodes per member, by chunk minima).  For each run: gangs placed
 inside one domain, gangs placed across domains (PREFERRED fallbacks) and gangs that failed.  Prints the device name and
 power limit with the figures; `--out FILE` also writes them as JSON."""
 import json
