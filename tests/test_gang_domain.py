@@ -32,22 +32,23 @@ def _i32(a):
     return None if a is None else np.ascontiguousarray(a, dtype=np.int32)
 
 
-def _W():
+def _W(W=None):
+    """The link-weight table W as int32[16]; None is the default table."""
     from oracle import oracle_b
-    return np.ascontiguousarray(oracle_b.DEFAULT_WEIGHTS, dtype=np.int32)
+    return np.ascontiguousarray(oracle_b.DEFAULT_WEIGHTS if W is None else W, dtype=np.int32)
 
 
 @pytest.fixture(scope="session")
 def twin():
-    """place(topo, free, pods, gang, gd, domain, mem=None, base=0) -> (keys, free_after)."""
+    """place(topo, free, pods, gang, gd, domain, mem=None, base=0, W=None) -> (keys, free_after)."""
     L = gang_domain_libs.twin()
 
-    def place(topo, free, pods, gang, gd, domain, mem=None, base=0):
+    def place(topo, free, pods, gang, gd, domain, mem=None, base=0, W=None):
         topo, pods, gang, gd, domain, mem = (_i32(a) for a in (topo, pods, gang, gd, domain, mem))
         f = np.array(free, dtype=np.int32, copy=True)
         keys = np.empty(len(pods), dtype=np.uint64)
         L.gang_domain_twin_place_batch(_p(topo), _p(f), _p(mem), len(f), base, _p(domain), _p(pods), _p(gang), _p(gd), len(pods),
-                                       _p(_W()), _p(keys, ctypes.c_uint64))
+                                       _p(_W(W)), _p(keys, ctypes.c_uint64))
         return keys, f
     return place
 
@@ -57,11 +58,11 @@ def gang_twin():
     """kgpu_place_batch_gang's twin (tests/gang_twin): the plain gang result."""
     L = cpu_libs.twin("gang")
 
-    def place(topo, free, pods, gang, mem=None, base=0):
+    def place(topo, free, pods, gang, mem=None, base=0, W=None):
         topo, pods, gang, mem = (_i32(a) for a in (topo, pods, gang, mem))
         f = np.array(free, dtype=np.int32, copy=True)
         keys = np.empty(len(pods), dtype=np.uint64)
-        L.gang_twin_place_batch(_p(topo), _p(f), _p(mem), len(f), base, _p(pods), _p(gang), len(pods), _p(_W()), _p(keys, ctypes.c_uint64))
+        L.gang_twin_place_batch(_p(topo), _p(f), _p(mem), len(f), base, _p(pods), _p(gang), len(pods), _p(_W(W)), _p(keys, ctypes.c_uint64))
         return keys, f
     return place
 
@@ -99,8 +100,9 @@ def random_batch(P, seed, share=0.6):
 
 
 # ---- a Python brute force of the definition ------------------------------------------------------------------------------
-def brute_force(topo, free, pods, gang, gd, domain, mem=None, base=0):
+def brute_force(topo, free, pods, gang, gd, domain, mem=None, base=0, W=None):
     from oracle import oracle_b
+    W = _W(W)
     F = [int(x) for x in free]
     N = len(F)
     keys = np.full(len(pods), NO_FIT, dtype=np.uint64)
@@ -108,7 +110,7 @@ def brute_force(topo, free, pods, gang, gd, domain, mem=None, base=0):
     def nkey(n, mask, k, need):
         if mem is not None and need > 0:
             mask &= sum(1 << i for i in range(8) if mem[n][i] >= need)
-        return oracle_b.node_key(topo[n], mask, k)
+        return oracle_b.node_key(topo[n], mask, k, W)
 
     def place(members, state, nodes):
         """members in order on a copy of state over `nodes`: (keys, state, cost), or None if one misses."""
@@ -373,12 +375,12 @@ def emu():
     return gang_domain_libs.emu()
 
 
-def emu_place(emu, topo, free, pods, gang, gd, domain, mem=None, base=0):
+def emu_place(emu, topo, free, pods, gang, gd, domain, mem=None, base=0, W=None):
     topo, pods, gang, gd, domain, mem = (_i32(a) for a in (topo, pods, gang, gd, domain, mem))
     f = np.array(free, dtype=np.int32, copy=True)
     keys = np.empty(len(pods), dtype=np.uint64)
     steps = emu.emu_place_batch_gang_domain(_p(topo), _p(f), _p(mem), len(f), base, _p(domain), _p(pods), _p(gang), _p(gd), len(pods),
-                                            _p(_W()), _p(keys, ctypes.c_uint64))
+                                            _p(_W(W)), _p(keys, ctypes.c_uint64))
     assert steps >= 0
     return keys, f, steps
 

@@ -27,7 +27,7 @@ _PLACE = [_i32p, _i32p, _i32p, _i64, _i64, _i32p, _int, _i32p, _i32p, _i32p, _i3
 # ---- the CPU libraries ------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="session")
 def twin():
-    """place(topo, free, pods, gang, gd, gl, domain[L, N], mem=None, base=0) -> (keys, free_after)."""
+    """place(topo, free, pods, gang, gd, gl, domain[L, N], mem=None, base=0, W=None) -> (keys, free_after)."""
     L = cpu_libs.twin("gang_domain_levels")
     L.levels_twin_place_batch.restype, L.levels_twin_place_batch.argtypes = None, _PLACE
     return lambda *a, **kw: _run(L.levels_twin_place_batch, *a, **kw)[:2]
@@ -35,16 +35,17 @@ def twin():
 
 @pytest.fixture(scope="session")
 def one_level_twin():
-    """kgpu_place_batch_gang_domain's twin: place(topo, free, pods, gang, gd, domain[N], mem=None) -> (keys, free_after)."""
+    """kgpu_place_batch_gang_domain's twin: place(topo, free, pods, gang, gd, domain[N], mem=None, base=0, W=None) ->
+    (keys, free_after)."""
     import gang_domain_libs
     L = gang_domain_libs.twin()
 
-    def place(topo, free, pods, gang, gd, domain, mem=None, base=0):
+    def place(topo, free, pods, gang, gd, domain, mem=None, base=0, W=None):
         topo, pods, gang, gd, domain, mem = (_i32(a) for a in (topo, pods, gang, gd, domain, mem))
         f = np.array(free, dtype=np.int32, copy=True)
         keys = np.empty(len(pods), dtype=np.uint64)
         L.gang_domain_twin_place_batch(_p(topo), _p(f), _p(mem), len(f), base, _p(domain), _p(pods), _p(gang), _p(gd), len(pods),
-                                       _p(_W()), _p(keys, ctypes.c_uint64))
+                                       _p(_W(W)), _p(keys, ctypes.c_uint64))
         return keys, f
     return place
 
@@ -53,11 +54,11 @@ def one_level_twin():
 def gang_twin():
     L = cpu_libs.twin("gang")
 
-    def place(topo, free, pods, gang):
+    def place(topo, free, pods, gang, W=None):
         topo, pods, gang = (_i32(a) for a in (topo, pods, gang))
         f = np.array(free, dtype=np.int32, copy=True)
         keys = np.empty(len(pods), dtype=np.uint64)
-        L.gang_twin_place_batch(_p(topo), _p(f), None, len(f), 0, _p(pods), _p(gang), len(pods), _p(_W()), _p(keys, ctypes.c_uint64))
+        L.gang_twin_place_batch(_p(topo), _p(f), None, len(f), 0, _p(pods), _p(gang), len(pods), _p(_W(W)), _p(keys, ctypes.c_uint64))
         return keys, f
     return place
 
@@ -75,18 +76,18 @@ def emu():
     return L
 
 
-def _run(fn, topo, free, pods, gang, gd, gl, domain, mem=None, base=0):
+def _run(fn, topo, free, pods, gang, gd, gl, domain, mem=None, base=0, W=None):
     topo, pods, gang, gd, gl, mem = (_i32(a) for a in (topo, pods, gang, gd, gl, mem))
     dom = None if domain is None else _i32(np.atleast_2d(domain))
     f = np.array(free, dtype=np.int32, copy=True)
     keys = np.empty(len(pods), dtype=np.uint64)
     rc = fn(_p(topo), _p(f), _p(mem), len(f), base, _p(dom), 1 if dom is None else dom.shape[0], _p(pods), _p(gang), _p(gd), _p(gl),
-            len(pods), _p(_W()), _p(keys, ctypes.c_uint64))
+            len(pods), _p(_W(W)), _p(keys, ctypes.c_uint64))
     return keys, f, rc
 
 
 # ---- a brute force of the climb, on test_gang_domain's brute force of one level ------------------------------------------
-def brute_force_levels(topo, free, pods, gang, gd, gl, domain, mem=None, base=0):
+def brute_force_levels(topo, free, pods, gang, gd, gl, domain, mem=None, base=0, W=None):
     """Run by run on the running state: a constrained gang is test_gang_domain.brute_force with REQUIRED on level 0, 1,
     ... gang_level until one places it; else NO_FIT (REQUIRED) or brute_force's plain gang (PREFERRED)."""
     F = np.array(free, dtype=np.int32)
@@ -98,7 +99,7 @@ def brute_force_levels(topo, free, pods, gang, gd, gl, domain, mem=None, base=0)
             e += 1
         sl = slice(p, e)
         one = lambda mode, lv: brute_force(topo, F, pods[sl], gang[sl], np.full(e - p, mode, np.int32),
-                                           domain[lv] if lv >= 0 else np.full(len(F), -1, np.int32), mem=mem, base=base)
+                                           domain[lv] if lv >= 0 else np.full(len(F), -1, np.int32), mem=mem, base=base, W=W)
         res = None
         if gd[p] != 0:
             for lv in range(int(gl[p]) + 1):
@@ -266,10 +267,10 @@ def test_table_builder_refuses(emu):
 
 
 # ---- the launch plan on the CPU -----------------------------------------------------------------------------------------------
-def emu_place(emu, topo, free, pods, gang, gd, gl, domain, mem=None, base=0, force_chunked=False):
+def emu_place(emu, topo, free, pods, gang, gd, gl, domain, mem=None, base=0, force_chunked=False, W=None):
     """force_chunked: every level walked by chunk minima, whatever its domains' size."""
     fn = lambda *a: emu.emu_place_batch_gang_levels(*a, int(force_chunked))
-    keys, f, launches = _run(fn, topo, free, pods, gang, gd, gl, domain, mem=mem, base=base)
+    keys, f, launches = _run(fn, topo, free, pods, gang, gd, gl, domain, mem=mem, base=base, W=W)
     assert launches >= 0
     return keys, f, launches
 

@@ -35,9 +35,10 @@ def _i32(a):
     return None if a is None else np.ascontiguousarray(a, dtype=np.int32)
 
 
-def _W():
+def _W(W=None):
+    """The link-weight table W as int32[16]; None is the default table."""
     from oracle import oracle_b
-    return np.ascontiguousarray(oracle_b.DEFAULT_WEIGHTS, dtype=np.int32)
+    return np.ascontiguousarray(oracle_b.DEFAULT_WEIGHTS if W is None else W, dtype=np.int32)
 
 
 def _out(P):
@@ -53,43 +54,44 @@ def _state(free, hold):
 def plans():
     """(domain_plan, gang_plan, snapshot).  domain_plan(topo, free, hold, mem, domain, pods, lvl, gang, gd, base=0) ->
     (keys, victims, F, H) with the final working state; gang_plan(topo, free, hold, mem, pods, lvl, gang, base=0) ->
-    (keys, victims) is preempt_plan_gang_twin; snapshot(topo, free, hold, mem, pods, lvl, base=0) is preempt_twin_batch."""
+    (keys, victims) is preempt_plan_gang_twin; snapshot(topo, free, hold, mem, pods, lvl, base=0) is preempt_twin_batch.
+    Each takes W=None, the link-weight table (None: the default)."""
     L = preempt_plan_domain_libs.twin()
     nt = os.cpu_count() or 1
 
-    def domain_plan(topo, free, hold, mem, domain, pods, lvl, gang, gd, base=0):
+    def domain_plan(topo, free, hold, mem, domain, pods, lvl, gang, gd, base=0, W=None):
         topo, mem, domain, pods, lvl, gang, gd = (_i32(a) for a in (topo, mem, domain, pods, lvl, gang, gd))
         F, H = _state(free, hold)
         keys, vic = _out(len(pods))
         L.preempt_plan_domain_twin(_p(topo), _p(F), _p(mem), _p(H), len(F), base, _p(domain), _p(pods), _p(lvl), _p(gang), _p(gd),
-                                   len(pods), _p(_W()), nt, _p(keys, ctypes.c_uint64), _p(vic, ctypes.c_uint32))
+                                   len(pods), _p(_W(W)), nt, _p(keys, ctypes.c_uint64), _p(vic, ctypes.c_uint32))
         return keys, vic, F, H
 
-    def gang_plan(topo, free, hold, mem, pods, lvl, gang, base=0):
+    def gang_plan(topo, free, hold, mem, pods, lvl, gang, base=0, W=None):
         topo, free, hold, mem, pods, lvl, gang = (_i32(a) for a in (topo, free, hold, mem, pods, lvl, gang))
         keys, vic = _out(len(pods))
         L.preempt_plan_gang_twin(_p(topo), _p(free), _p(mem), _p(hold), len(free), base, _p(pods), _p(lvl), _p(gang), len(pods),
-                                 _p(_W()), nt, _p(keys, ctypes.c_uint64), _p(vic, ctypes.c_uint32))
+                                 _p(_W(W)), nt, _p(keys, ctypes.c_uint64), _p(vic, ctypes.c_uint32))
         return keys, vic
 
-    def snapshot(topo, free, hold, mem, pods, lvl, base=0):
+    def snapshot(topo, free, hold, mem, pods, lvl, base=0, W=None):
         topo, free, hold, mem, pods, lvl = (_i32(a) for a in (topo, free, hold, mem, pods, lvl))
         keys, vic = _out(len(pods))
-        L.preempt_twin_batch(_p(topo), _p(free), _p(mem), _p(hold), len(free), base, _p(pods), _p(lvl), len(pods), _p(_W()), 1,
+        L.preempt_twin_batch(_p(topo), _p(free), _p(mem), _p(hold), len(free), base, _p(pods), _p(lvl), len(pods), _p(_W(W)), 1,
                              _p(keys, ctypes.c_uint64), _p(vic, ctypes.c_uint32))
         return keys, vic
 
     return domain_plan, gang_plan, snapshot
 
 
-def k3_dry_run(topo, free, mem, domain, pods, gang, gd, base=0):
+def k3_dry_run(topo, free, mem, domain, pods, gang, gd, base=0, W=None):
     """kgpu_place_batch_gang_domain(KGPU_PLACE_DRY_RUN)'s keys, from K3's domain twin."""
     L = gang_domain_libs.twin()
     topo, mem, domain, pods, gang, gd = (_i32(a) for a in (topo, mem, domain, pods, gang, gd))
     f = np.array(free, np.int32, copy=True)
     keys = np.empty(len(pods), np.uint64)
     L.gang_domain_twin_place_batch(_p(topo), _p(f), _p(mem), len(f), base, _p(domain), _p(pods), _p(gang), _p(gd), len(pods),
-                                   _p(_W()), _p(keys, ctypes.c_uint64))
+                                   _p(_W(W)), _p(keys, ctypes.c_uint64))
     return keys
 
 
@@ -126,7 +128,7 @@ def random_batch(P, seed, share=0.6):
 
 
 # ---- a Python brute force of the definition ------------------------------------------------------------------------------
-def brute_force(snapshot, topo, free, hold, mem, domain, pods, lvl, gang, gd, base=0):
+def brute_force(snapshot, topo, free, hold, mem, domain, pods, lvl, gang, gd, base=0, W=None):
     """The definition, literally: every member is a single-pod snapshot call on (F, H) with the nodes outside the trial's
     domain masked out (no free GPU, nothing evictable), followed by the update rule; k = 0 takes the domain's lowest node."""
     F, H = _state(free, hold)
@@ -142,7 +144,7 @@ def brute_force(snapshot, topo, free, hold, mem, domain, pods, lvl, gang, gd, ba
             n = 0 if allowed is None else int(np.flatnonzero(allowed)[0])
             return np.uint64((base + n) << 8), 0, 0, 0
         Fm, Hm = (F, H) if allowed is None else (np.where(allowed, F, 0), np.where(allowed[:, None], H, -1))
-        kk, vv = snapshot(topo, Fm, Hm, mem, pods[q:q + 1], lvl[q:q + 1], base=base)
+        kk, vv = snapshot(topo, Fm, Hm, mem, pods[q:q + 1], lvl[q:q + 1], base=base, W=W)
         if kk[0] == NO_FIT:
             return None
         n, v = node_of(kk[0], base), int(vv[0])
@@ -533,12 +535,12 @@ def emu():
     return preempt_plan_domain_libs.emu()
 
 
-def emu_plan(emu, topo, free, hold, mem, domain, pods, lvl, gang, gd, base=0):
+def emu_plan(emu, topo, free, hold, mem, domain, pods, lvl, gang, gd, base=0, W=None):
     topo, mem, domain, pods, lvl, gang, gd = (_i32(a) for a in (topo, mem, domain, pods, lvl, gang, gd))
     F, H = _state(free, hold)
     keys, vic = _out(len(pods))
     steps = emu.emu_preempt_plan_gang_domain(_p(topo), _p(F), _p(mem), _p(H), len(F), base, _p(domain), _p(pods), _p(lvl), _p(gang),
-                                             _p(gd), len(pods), _p(_W()), _p(keys, ctypes.c_uint64), _p(vic, ctypes.c_uint32))
+                                             _p(gd), len(pods), _p(_W(W)), _p(keys, ctypes.c_uint64), _p(vic, ctypes.c_uint32))
     assert steps >= 0
     return keys, vic, F, H, steps
 
